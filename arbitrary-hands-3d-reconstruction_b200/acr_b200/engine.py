@@ -487,6 +487,14 @@ class Engine:
                                                    cnt.ctypes.data), "plan_profile")
         return {k: (float(ms[k]), int(cnt[k])) for k in range(16) if cnt[k]}
 
+    def profile_ops(self, image: torch.Tensor) -> np.ndarray:
+        """One serialised, event-bracketed pass: device ms of every launch, in the order of ``recs``."""
+        ms = np.zeros(self.num_launches, np.float32)
+        with torch.cuda.device(self.device):
+            L.check(self.lib.acr_b200_plan_profile_ops(self.plan, image.data_ptr(), self._stream(), ms.ctypes.data),
+                    "plan_profile_ops")
+        return ms
+
     @property
     def num_launches(self) -> int:
         return int(self.lib.acr_b200_plan_num_launches(self.plan))

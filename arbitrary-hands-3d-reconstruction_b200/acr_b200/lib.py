@@ -57,7 +57,7 @@ _lib: Optional[C.CDLL] = None
 
 EXPORTS = ["acr_b200_last_error", "acr_b200_version", "acr_b200_mano_model_floats", "acr_b200_mano_pack_model",
            "acr_b200_mano_forward", "acr_b200_mano_forward_gather", "acr_b200_gather_wait", "acr_b200_cam_trans", "acr_b200_preprocess", "acr_b200_one_euro_state_floats", "acr_b200_one_euro_smooth", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse",
-           "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_num_launches", "acr_b200_plan_destroy",
+           "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_profile_ops", "acr_b200_plan_num_launches", "acr_b200_plan_destroy",
            "acr_b200_run_op", "acr_b200_pack_conv"]
 
 
@@ -90,6 +90,7 @@ def load() -> C.CDLL:
                                          C.POINTER(vp)]
     lib.acr_b200_plan_run.argtypes = [vp, vp, vp]
     lib.acr_b200_plan_profile.argtypes = [vp, vp, vp, vp, vp]
+    lib.acr_b200_plan_profile_ops.argtypes = [vp, vp, vp, vp]
     lib.acr_b200_plan_num_launches.argtypes = [vp]
     lib.acr_b200_plan_destroy.argtypes = [vp]
     lib.acr_b200_plan_destroy.restype = None

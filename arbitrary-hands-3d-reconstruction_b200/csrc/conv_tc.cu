@@ -180,6 +180,9 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   if ((p.patch1 || p.s2x) && SA > 4) SA = 4;
   if (SA < 2) { set_error("conv_tc: shared memory plan does not fit (cout_pad %d, ck %d)", a.cout_pad, ck); delete pl; return ACR_B200_EINVAL; }
   p.SA = SA;
+  // ping-pong teams need every A load of a tile in the ring at once (conv_tc_kernel); the four-view stride-2 convs
+  // (9 loads per channel chunk) and the 16-channel-chunk patch convs with several chunks stay in lockstep
+  p.pingpong = (p.b_resident && nA <= SA) ? 1 : 0;
   pl->smem = fixed + p.b_region_bytes + (size_t)SA * p.a_stage_bytes;
   pl->grid = p.total_tiles * nsplit < num_sms() ? p.total_tiles * nsplit : num_sms();
   *out = pl;

@@ -22,8 +22,11 @@
 //   * Both land in shared memory in the canonical K-major swizzled layout (128B / 64B / 32B swizzle for CK = 64 / 32 / 16)
 //     that wgmma descriptors address directly.
 //   * Persistent CTAs (one per SM): warps 0..15 = the four consumer warpgroups (wgmma issue, then the epilogue straight
-//     from the accumulator registers: +bias (+residual) (+extra terms) (ReLU) -> 16-bit / fp32 NHWC); warp 16 = TMA
-//     producer, which runs ahead into the next tile's operands while the consumers finish the epilogue of this one.
+//     from the accumulator registers: +bias (+residual) (+extra terms) (ReLU) -> 16-bit / fp32 NHWC); warps 16..19 = the
+//     producer warpgroup, whose first warp issues the TMA loads and runs ahead into the next tile's operands.  The producer
+//     gives registers to the consumers (setmaxnreg).
+//   * Resident weights: the consumers run as two ping-pong teams by row group (warpgroups {0,1} and {2,3}), so one team's
+//     epilogue overlaps the other team's MMAs.  Streamed weights: all four warpgroups issue in lockstep.
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -84,6 +87,13 @@ __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+// arrive (without waiting) when pred != 0; one asm statement, so it may sit between wgmma commit and wait
+__device__ __forceinline__ void named_bar_arrive_if(int id, int nthreads, uint32_t pred) {
+  asm volatile("{\n.reg .pred p;\nsetp.ne.u32 p, %2, 0;\n@p bar.arrive %0, %1;\n}\n" ::"r"(id), "r"(nthreads), "r"(pred) : "memory");
+}
+// per-thread register budget of the executing warpgroup (warpgroup-collective)
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
 __device__ __forceinline__ uint64_t desc_lohi(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 
@@ -108,8 +118,17 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
 // four M = 64 blocks and three (nine) taps.
 constexpr int TILE_Y = 16, TILE_X = 16, HALF_X = 8;
 constexpr int CONSUMER_WARPS = 16;                 // four warpgroups, one M = 64 block of the super-tile each
-constexpr int PRODUCER_WARP = CONSUMER_WARPS;
-constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 1);
+constexpr int PRODUCER_WARP = CONSUMER_WARPS;      // first warp of the producer warpgroup: the TMA issuer
+constexpr int TC_THREADS = 32 * (CONSUMER_WARPS + 4);
+// Register split: 640 threads launch with 96 registers each (61440 of the SM's 64K).  The producer warpgroup drops to 32,
+// which lets the consumers rise to 112 (16 x 32 x 112 + 4 x 32 x 32 = 61440): room for a 64-register accumulator (NT = 128)
+// without spilling.
+constexpr int PRODUCER_REGS = 32, CONSUMER_REGS = 112;
+static_assert(CONSUMER_WARPS * 32 * CONSUMER_REGS + 4 * 32 * PRODUCER_REGS <= (65536 / TC_THREADS) / 8 * 8 * TC_THREADS,
+              "setmaxnreg split exceeds the launch allocation");
+// named barriers of the ping-pong teams (ids 1..4 are the TMA-store epilogue's per-warpgroup barriers): barrier
+// TEAM_BAR + t completes when team t may issue its next tile
+constexpr int TEAM_BAR = 5;
 constexpr int MAX_NSUB = 128;                      // accumulator columns per warpgroup (64 fp32 registers per thread)
 constexpr int SMEM_BUDGET = 224 * 1024;            // of the 227 KB a Hopper block may opt into
 
@@ -130,6 +149,7 @@ struct ConvTcParams {
                         // one may extend past cout_pad: those columns are computed from zero / unused weights and not stored)
   int xpair;    // x-paired 32->32 conv run as 64->64 (see below): side taps are quarter blocks
   int patch_mode, b_resident, SA, SB;
+  int pingpong;   // resident weights and a tile's A loads fit in the ring: the consumer teams alternate (see the kernel)
   int patch1;   // MODE_P1: ONE 24-wide haloed box per channel chunk, kx shifts = unaligned descriptor starts
   int s2x;      // MODE_S2X: 3x3 stride-2 conv of a dense 32-channel tensor read as x-pairs: two row-parity boxes per tile
   uint32_t a_stage_bytes, b_block_bytes, b_region_bytes;
@@ -215,9 +235,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   // nothing the previous kernel produces
   pdl_launch_dependents();
 
-  if (warp == PRODUCER_WARP) {
-    // ===================================================================== TMA producer
-    // (whole warp stays converged; one elected lane issues)
+  if (warp >= CONSUMER_WARPS) {
+    // ===================================================================== TMA producer warpgroup
+    // (one warp issues: it stays converged and one elected lane issues; the other three only give up registers)
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp != PRODUCER_WARP) return;
     if (P.b_resident && elect_one_sync()) {  // whole weight tensor once per CTA
       const int nblk = P.taps * P.cchunks;
       mbar_expect_tx(bres_bar, (uint32_t)nblk * P.b_block_bytes);
@@ -288,6 +310,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   // (wgmma.wait_group 1); only then are the operand stages it read handed back to the producer.  Between the wgmmas there
   // is no C++ branch or call (waits and arrivals are single asm statements, NT and the tap pattern are compile-time):
   // otherwise ptxas serialises the wgmmas.
+  //
+  // Ping-pong (resident weights): team rg (warpgroups 2 rg, 2 rg + 1) issues ALL wgmmas of a tile, then hands the turn
+  // to the other team and only then waits for its own MMAs and runs its epilogue, which so overlaps the other team's
+  // MMAs.  Barrier TEAM_BAR + t: team t waits on it (bar.sync) before a tile, the other team arrives after issuing its
+  // own tile.  Team 1 pre-arrives once so that team 0 goes first, and skips its arrival after its last tile, so every
+  // barrier phase completes by kernel exit.  Both teams read the same A stages, which the producer refills only after
+  // all 16 consumer warps released them, so the A ring must hold all loads of a tile (P.pingpong, set by the plan):
+  // otherwise the first team would wait for a stage that only the second team, still waiting for its turn, can free.
+  // Streamed weights stay in lockstep: staggered teams would read every streamed B block a team phase apart, so the
+  // B ring would have to hold a whole tile of weights.
+  constexpr bool PINGPONG = RESIDENT;
+  const bool pingpong = PINGPONG && P.pingpong != 0;
+  setmaxnreg_inc<CONSUMER_REGS>();
   const int wg = warp >> 2, wq = warp & 3;
   const int h = wg & 1, rg = wg >> 1;           // half (left / right 8 columns), row group (image rows 0..7 / 8..15)
   if (RESIDENT) mbar_wait_parity(bres_bar, 0);
@@ -346,7 +381,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 
   int sa = 0, sb = 0;
   uint32_t pha = 0, phb = 0;
-  for (int vt = blockIdx.x; vt < P.total_tiles * P.nsplit; vt += gridDim.x) {
+  uint32_t xa_bar[3];   // x-paired form: the three A stages of the tile, released once its MMAs completed
+  const int nvt = P.total_tiles * P.nsplit;
+  if (pingpong && rg == 1) named_bar_arrive_if(TEAM_BAR, 512, 1u);
+  for (int vt = blockIdx.x; vt < nvt; vt += gridDim.x) {
+    if (pingpong) named_bar_sync(TEAM_BAR + rg, 512);
     scale = 0;
     // resident weights hold all N rows: this virtual tile multiplies rows [n_off, n_off + NT)
     const uint32_t b_lo_base = b_lo_base0 + (RESIDENT ? (uint32_t)((vt % P.nsplit) * nsub) * (Cfg::kRowBytes >> 4) : 0u);
@@ -402,31 +441,25 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         if (++sa == SA) { sa = 0; pha ^= 1u; }
       }
     } else if (PATCH && XPAIR) {
-      // x-paired (resident weights): the three kx boxes of a chunk, then its nine taps ky-major with kx 1, 0, 2 -- the
-      // summation order of the single-box form -- in one group
-      for (int cc = 0; cc < cchunks; ++cc) {
-        uint32_t a_lo[3], a_bar[3];
+      // x-paired (resident weights, one 64-channel chunk: conv_tc_prepare): the three kx boxes, then the nine taps
+      // ky-major with kx 1, 0, 2 -- the summation order of the single-box form -- in one group
+      uint32_t a_lo[3];
 #pragma unroll
-        for (int i = 0; i < 3; ++i) {   // box i holds kx = patch_kx(i) = 1, 0, 2
-          mbar_wait_parity(fullA(sa), pha);
-          a_lo[i] = a_lo_base + (uint32_t)sa * a_stage16;
-          a_bar[i] = emptyA(sa);
-          if (++sa == SA) { sa = 0; pha ^= 1u; }
-        }
-        wgmma_fence();
-#pragma unroll
-        for (int ky = 0; ky < 3; ++ky)
-#pragma unroll
-          for (int i = 0; i < 3; ++i) {
-            const int kx = i == 0 ? 1 : (i == 1 ? 0 : 2);
-            issue(a_lo[i] + (uint32_t)ky * pitch16, b_lo_base + (uint32_t)((ky * 3 + kx) * cchunks + cc) * b_block16, kx);
-          }
-        wgmma_commit();
-        wgmma_wait<0>();
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 3; ++i) mbar_arrive_if(a_bar[i], is_lane0);
+      for (int i = 0; i < 3; ++i) {   // box i holds kx = patch_kx(i) = 1, 0, 2
+        mbar_wait_parity(fullA(sa), pha);
+        a_lo[i] = a_lo_base + (uint32_t)sa * a_stage16;
+        xa_bar[i] = emptyA(sa);
+        if (++sa == SA) { sa = 0; pha ^= 1u; }
       }
+      wgmma_fence();
+#pragma unroll
+      for (int ky = 0; ky < 3; ++ky)
+#pragma unroll
+        for (int i = 0; i < 3; ++i) {
+          const int kx = i == 0 ? 1 : (i == 1 ? 0 : 2);
+          issue(a_lo[i] + (uint32_t)ky * pitch16, b_lo_base + (uint32_t)(ky * 3 + kx) * b_block16, kx);
+        }
+      wgmma_commit();
     } else if (PATCH) {
       // one A stage per (channel chunk, kx): rows y0-1 .. y0+16, the three ky taps are 16-pixel row shifts
       for (int cc = 0; cc < cchunks; ++cc) {
@@ -465,8 +498,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
         }
       }
     }
+    // every wgmma of this tile is issued: the other team may issue its tile while this one's complete
+    if (PINGPONG) named_bar_arrive_if(TEAM_BAR + (rg ^ 1), 512, (pingpong && (rg == 0 || vt + (int)gridDim.x < nvt)) ? 1u : 0u);
     wgmma_wait<0>();
     release();
+    if (XPAIR) {
+#pragma unroll
+      for (int i = 0; i < 3; ++i) mbar_arrive_if(xa_bar[i], is_lane0);
+    }
     wgmma_acc_fence<NT / 2>(acc);
 
     // ---------------------------------------------------------------- epilogue, straight from the register fragment

@@ -283,10 +283,8 @@ extern "C" int acr_b200_plan_run(acr_b200_plan* p, const void* image, void* stre
   return ACR_B200_OK;
 }
 
-extern "C" int acr_b200_plan_profile(acr_b200_plan* p, const void* image, void* stream, float* ms_by_kind,
-                                     int32_t* n_by_kind) {
-  ACR_CHECK_ARG(p && image && ms_by_kind && n_by_kind, "plan_profile: bad arguments");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+// one serialised pass with an event after every op: device milliseconds of op i into ms_by_op[i]
+static int profile_ops(acr_b200_plan* p, const void* image, cudaStream_t st, float* ms_by_op) {
   const int n = (int)p->ops.size();
   std::vector<cudaEvent_t> ev(n + 1);
   for (auto& e : ev) ACR_CHECK_CUDA(cudaEventCreate(&e));
@@ -297,17 +295,33 @@ extern "C" int acr_b200_plan_profile(acr_b200_plan* p, const void* image, void* 
     if (rc == ACR_B200_OK && cudaEventRecord(ev[i + 1], st) != cudaSuccess) rc = ACR_B200_ECUDA;
   }
   if (rc == ACR_B200_OK && cudaStreamSynchronize(st) != cudaSuccess) { set_error("plan_profile: sync failed: %s", cudaGetErrorString(cudaGetLastError())); rc = ACR_B200_ECUDA; }
-  if (rc == ACR_B200_OK) {
-    for (int k = 0; k < 16; ++k) { ms_by_kind[k] = 0.f; n_by_kind[k] = 0; }
+  if (rc == ACR_B200_OK)
     for (int i = 0; i < n; ++i) {
-      float ms = 0.f;
-      cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-      const int k = p->ops[i].kind & 15;
-      ms_by_kind[k] += ms; n_by_kind[k] += 1;
+      ms_by_op[i] = 0.f;
+      cudaEventElapsedTime(&ms_by_op[i], ev[i], ev[i + 1]);
     }
-  }
   for (auto& e : ev) cudaEventDestroy(e);
   return rc;
+}
+
+extern "C" int acr_b200_plan_profile(acr_b200_plan* p, const void* image, void* stream, float* ms_by_kind,
+                                     int32_t* n_by_kind) {
+  ACR_CHECK_ARG(p && image && ms_by_kind && n_by_kind, "plan_profile: bad arguments");
+  std::vector<float> ms(p->ops.size());
+  const int rc = profile_ops(p, image, static_cast<cudaStream_t>(stream), ms.data());
+  if (rc == ACR_B200_OK) {
+    for (int k = 0; k < 16; ++k) { ms_by_kind[k] = 0.f; n_by_kind[k] = 0; }
+    for (size_t i = 0; i < ms.size(); ++i) {
+      const int k = p->ops[i].kind & 15;
+      ms_by_kind[k] += ms[i]; n_by_kind[k] += 1;
+    }
+  }
+  return rc;
+}
+
+extern "C" int acr_b200_plan_profile_ops(acr_b200_plan* p, const void* image, void* stream, float* ms_by_op) {
+  ACR_CHECK_ARG(p && image && ms_by_op, "plan_profile_ops: bad arguments");
+  return profile_ops(p, image, static_cast<cudaStream_t>(stream), ms_by_op);
 }
 
 extern "C" int acr_b200_plan_num_launches(const acr_b200_plan* p) { return p ? (int)p->ops.size() : 0; }

@@ -272,6 +272,9 @@ int acr_b200_plan_run(acr_b200_plan* plan, const void* image, void* stream);
  * (host arrays, indexed by ACR_OP_*).  Synchronises `stream`.  Used by bench.py for the roofline. */
 int acr_b200_plan_profile(acr_b200_plan* plan, const void* image, void* stream, float* ms_by_kind,
                           int32_t* n_by_kind);
+/* The same serialised, event-bracketed pass, but writes the device milliseconds of op i into ms_by_op[i]
+ * (host array of plan_num_launches floats, in plan order).  Synchronises `stream`.  Per-layer tables. */
+int acr_b200_plan_profile_ops(acr_b200_plan* plan, const void* image, void* stream, float* ms_by_op);
 /* Number of kernel launches one plan_run issues (for bench.py's gpu_launches).            */
 int acr_b200_plan_num_launches(const acr_b200_plan* plan);
 void acr_b200_plan_destroy(acr_b200_plan* plan);

@@ -1,0 +1,142 @@
+#!/usr/bin/env python
+"""Per-layer-class table of the conv launch set of one bench step, timed with CUDA events (Engine.profile_ops):
+    python tools/conv_layers.py [--batch 256] [--warmup 2] [--passes 5]
+    python tools/conv_layers.py --dry-run        shapes, FLOP, bytes and floors only (no GPU needed)
+
+Conv launches are grouped by (cin, cout, k, s, H_in, residual).  Per class: launches, device ms (the median of every
+launch over the profiled passes, summed), TFLOP/s, algorithmic GB/s (input + output (+ residual) (+ extra terms) once),
+the compute floor (FLOP over SMs x 4096 dense bf16 FLOP/clk x the SM clock sampled during the passes), the HBM floor
+(algorithmic bytes over --hbm-gbs) and measured time over the larger floor.  `weights KB` is the layer's bf16 weight
+tensor (cout x cin x k x k): layers whose packed weights do not fit in shared memory next to the operand stages stream
+them (conv_tc_prepare), the others keep them resident.
+The card name, power limit and SM clock are read in the same run."""
+import argparse
+import collections
+import os
+import subprocess
+import sys
+import threading
+
+ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
+sys.path.insert(0, os.path.join(ROOT, "arbitrary-hands-3d-reconstruction_b200"))
+import numpy as np  # noqa: E402
+
+from acr_b200 import lib as L  # noqa: E402
+from acr_b200.engine import Engine  # noqa: E402
+
+FLOP_PER_CLK_SM = 4096   # dense bf16 wgmma, per SM and clock (H100)
+
+
+def smi(query, index=0):
+    out = subprocess.run(["nvidia-smi", f"--query-gpu={query}", "--format=csv,noheader,nounits", "-i", str(index)],
+                         capture_output=True, text=True, timeout=10).stdout
+    return [c.strip() for c in out.strip().split(",")]
+
+
+class ClockSampler(threading.Thread):
+    """SM clock (MHz) sampled every 0.2 s while the profiled passes run."""
+
+    def __init__(self, index):
+        super().__init__(daemon=True)
+        self.index, self.mhz, self.done = index, [], threading.Event()
+
+    def run(self):
+        while not self.done.is_set():
+            try:
+                self.mhz.append(float(smi("clocks.sm", self.index)[0]))
+            except Exception:   # noqa: BLE001 -- a missed sample only shortens the list
+                pass
+            self.done.wait(0.2)
+
+    def stop(self):
+        self.done.set()
+        self.join(timeout=5)
+        return float(np.median(self.mhz)) if self.mhz else None
+
+
+def conv_classes(recs, batch):
+    """[(key, [rec indices], GFLOP, algorithmic MB, weights KB)] of the conv launches, in plan order of first use."""
+    agg = collections.OrderedDict()
+    for i, r in enumerate(recs):
+        if r["kind"] != L.OP_CONV:
+            continue
+        x, y, at = r["ins"][0], r["out"], r["attrs"]
+        cin = 109 if "fold_side" in at else (27 if "stem" in at else x.C)   # real input channels of the GEMM
+        key = (cin, y.C, at["k"], at["s"], x.H, bool(at["residual"]))
+        a = agg.setdefault(key, [[], 0.0, 0.0, 0.0])
+        a[0].append(i)
+        a[1] += 2.0 * y.H * y.W * y.C * cin * at["k"] ** 2 * batch / 1e9
+        nbytes = batch * (x.H * x.W * x.C * 2 + y.H * y.W * y.C * (4 if y.dtype == "f32" else 2) * (2 if at["residual"] else 1))
+        if at.get("extra"):
+            nbytes += sum(batch * t.H * t.W * t.C * 2 for t in r["ins"][1:])
+        a[2] += nbytes / 1e6
+        a[3] = y.C * cin * at["k"] ** 2 * 2 / 1024
+    return [(k, *v) for k, v in agg.items()]
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--warmup", type=int, default=2, help="unrecorded profiled passes first")
+    ap.add_argument("--passes", type=int, default=5, help="profiled passes; every launch's median is used")
+    ap.add_argument("--hbm-gbs", type=float, default=3000.0, help="HBM bandwidth of the floor (GB/s)")
+    ap.add_argument("--sm-mhz", type=float, default=None, help="SM clock of the compute floor (default: sampled; 1600 dry)")
+    ap.add_argument("--sms", type=int, default=132)
+    ap.add_argument("--dry-run", action="store_true", help="no GPU: shapes, FLOP, bytes and floors without times")
+    args = ap.parse_args()
+
+    ms_op = None
+    if args.dry_run:
+        eng = Engine(None, args.batch, "cpu", dry_run=True)
+        mhz = args.sm_mhz or 1600.0
+        print(f"dry run (no GPU): batch {args.batch}, floors at {args.sms} SMs x {mhz:.0f} MHz and {args.hbm_gbs:.0f} GB/s")
+    else:
+        import torch
+        from acr_b200.synth import load_bn_calibration, synth_state_dict
+        dev = torch.device("cuda", torch.cuda.current_device())
+        name, plimit = smi("name,power.limit", dev.index)[:2]
+        sd = synth_state_dict(0, bn_stats=load_bn_calibration(0))
+        eng = Engine(sd, args.batch, dev, torch.bfloat16, 512)
+        frames = torch.randint(0, 256, (args.batch, 512, 512, 3), generator=torch.Generator().manual_seed(1000),
+                               dtype=torch.uint8).to(dev)
+        for _ in range(args.warmup):
+            eng.profile_ops(frames)
+        sampler = ClockSampler(dev.index)
+        sampler.start()
+        runs = np.stack([eng.profile_ops(frames) for _ in range(args.passes)])
+        sampled = sampler.stop()
+        ms_op = np.median(runs, axis=0)
+        mhz = args.sm_mhz or sampled or 1600.0
+        print(f"{name}, power limit {plimit} W, SM clock {sampled if sampled else 'n/a'} MHz (median during the passes); "
+              f"batch {args.batch}, median of {args.passes} passes after {args.warmup} warm-up; "
+              f"floors at {args.sms} SMs x {mhz:.0f} MHz and {args.hbm_gbs:.0f} GB/s")
+
+    peak_tflops = args.sms * FLOP_PER_CLK_SM * mhz * 1e6 / 1e12
+    rows = []
+    for key, idx, gflop, mb, wkb in conv_classes(eng.recs, args.batch):
+        t_c, t_m = gflop / peak_tflops, mb / args.hbm_gbs       # ms
+        ms = float(ms_op[idx].sum()) if ms_op is not None else None
+        rows.append((key, len(idx), wkb, gflop, mb, t_c, t_m, ms))
+    rows.sort(key=lambda r: -(r[7] if r[7] is not None else max(r[5], r[6])))
+    head = "| cin | cout | k | s | H_in | res | n | weights KB | GFLOP | MB | compute floor ms | HBM floor ms | bound |"
+    if ms_op is not None:
+        head += " ms | TFLOP/s | GB/s | x floor |"
+    print(head + "\n" + "|" + "---:|" * 5 + "---|" + "---:|" * 6 + "---|" + ("---:|" * 4 if ms_op is not None else ""))
+    for key, n, wkb, gflop, mb, t_c, t_m, ms in rows:
+        line = (f"| {key[0]} | {key[1]} | {key[2]} | {key[3]} | {key[4]} | {'y' if key[5] else ''} | {n} | {wkb:.0f} | "
+                f"{gflop:.1f} | {mb:.0f} | {t_c:.2f} | {t_m:.2f} | {'compute' if t_c >= t_m else 'HBM'} |")
+        if ms is not None:
+            line += f" {ms:.2f} | {gflop / ms:.0f} | {mb / ms:.0f} | {ms / max(t_c, t_m):.1f} |"
+        print(line)
+    tc, tm = sum(r[5] for r in rows), sum(r[6] for r in rows)
+    tf = sum(max(r[5], r[6]) for r in rows)
+    tail = (f"\n{sum(r[1] for r in rows)} conv launches, {sum(r[3] for r in rows):.0f} GFLOP, {sum(r[4] for r in rows) / 1e3:.1f} GB; "
+            f"floors: compute {tc:.1f} ms, HBM {tm:.1f} ms, sum of per-class max {tf:.1f} ms")
+    if ms_op is not None:
+        t = sum(r[7] for r in rows)
+        tail += f"; measured {t:.2f} ms ({sum(r[3] for r in rows) / t:.0f} TFLOP/s, {t / tf:.1f}x the floor)"
+    print(tail)
+
+
+if __name__ == "__main__":
+    main()

@@ -1,5 +1,6 @@
 """Per-kernel SASS audit of lib/libacr_b200.so: which kernels carry warpgroup MMA (HGMMA), TMA (UTMALDG / UTMASTG),
-mbarrier (SYNCS), warp-level MMA (HMMA) or system-scope stores.  Needs no GPU: cuobjdump -sass.
+mbarrier (SYNCS), warp-level MMA (HMMA), system-scope stores, or local-memory (spill) traffic (LDL / STL).  Needs no GPU:
+cuobjdump -sass.
     python tools/sass_audit.py [lib.so]  ->  markdown table on stdout"""
 import collections
 import os
@@ -10,7 +11,7 @@ import sys
 ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 LIB = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "arbitrary-hands-3d-reconstruction_b200", "lib", "libacr_b200.so")
 CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
-MNEMONICS = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "STG.E.128.STRONG.SYS", "LDGSTS"]
+MNEMONICS = ["HGMMA", "UTMALDG", "UTMASTG", "SYNCS", "HMMA", "STG.E.128.STRONG.SYS", "LDGSTS", "LDL", "STL", "USETMAXREG"]
 
 
 def demangle(names):
