@@ -14,7 +14,9 @@ from typing import Optional, Sequence
 project_dir = os.path.abspath(os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 
 _DEFAULTS = dict(
-    tab="ACR_hrnet_internet", backbone="hrnet",          # config.py:95 (flag is only a log tag, SURVEY F1)
+    tab="ACR_hrnet_internet", backbone="hrnet",          # config.py:95 ("resnet50 or hrnet"; only a log tag there, SURVEY F1):
+                                                          # values starting with "resnet" select the ResNet-50 trunk
+                                                          # (backbone_kind), every other value the HRNet trunk
     model_precision="bf16",                               # reference: fp32|fp16 (config.py:96); here bf16|fp16 = tensor-core
                                                           # plans, fp32 = the (slow, reference-accurate) validation plan
     hrnet_width=32,                                        # 32 = the reference's HRNet-W32 (the only trunk it contains); 48 = the
@@ -71,3 +73,10 @@ class ConfigContext(object):
 
 def args() -> argparse.Namespace:
     return ConfigContext.parsed_args
+
+
+def backbone_kind(ns: Optional[argparse.Namespace] = None) -> str:
+    """The trunk a configuration selects: "resnet50" for ``backbone`` values starting with "resnet" (the reference
+    documents "resnet50 or hrnet", configs/demo.yml carries 'resnet'), "hrnet" for every other value."""
+    ns = ns if ns is not None else args()
+    return "resnet50" if str(getattr(ns, "backbone", "hrnet")).lower().startswith("resnet") else "hrnet"

@@ -12,7 +12,7 @@ from collections import OrderedDict
 import torch
 import torch.nn as nn
 
-from acr.config import args
+from acr.config import args, backbone_kind
 from acr.result_parser import ResultParser
 from acr_b200.engine import Engine
 from acr_b200.netspec import WIDTHS, WIDTHS_W48, build_acr_spec
@@ -81,8 +81,10 @@ class LazyOutputs(dict):
 class ACR(nn.Module):
     def __init__(self, **kwargs):
         super().__init__()
+        # args().backbone starting with 'resnet': the ResNet-50 trunk (netspec.build_acr_spec); otherwise HRNet-W32 / W48
+        self._backbone = backbone_kind()
         self._widths = {32: WIDTHS, 48: WIDTHS_W48}[int(getattr(args(), 'hrnet_width', 32))]
-        self._spec = build_acr_spec(args().input_size, widths=self._widths)
+        self._spec = build_acr_spec(args().input_size, widths=self._widths, backbone=self._backbone)
         g = torch.Generator().manual_seed(0)
         for key, (shape, kind) in self._spec.params.items():
             if kind == 'bn_nbt':
@@ -146,7 +148,7 @@ class ACR(nn.Module):
             self._engines.move_to_end(key)
             return self._engines[key]
         eng = Engine(self.state_dict(), batch, dev, dt, args().input_size, debug_ref_conv=self.debug_ref_conv,
-                     head_only=head_only, weights=self._blobs.get(bkey), widths=self._widths)
+                     head_only=head_only, weights=self._blobs.get(bkey), widths=self._widths, backbone=self._backbone)
         self._blobs[bkey] = eng.weights
         self._engines[key] = eng
         while len(self._engines) > max(1, self.max_engines):

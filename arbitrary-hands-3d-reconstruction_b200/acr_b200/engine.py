@@ -85,6 +85,20 @@ class _Arena:
         self.free = merged
 
 
+def deconv_parity_weights(w: np.ndarray) -> np.ndarray:
+    """ConvTranspose2d(k4, s2, p1) weight (cin, cout, 4, 4) -> the four 2x2 convs it is made of, (4, cout, cin, 2, 2) OIHW.
+    Output pixel (2m+py, 2n+px) = sum over taps (ty, tx) of x[m + py + ty - 1, n + px + tx - 1] . w[:, :, 3-py-2ty, 3-px-2tx]:
+    parity p = py*2 + px, tap (ty, tx) reads the input at offset (py + ty - 1, px + tx - 1)."""
+    cin, cout = w.shape[:2]
+    out = np.zeros((4, cout, cin, 2, 2), np.float32)
+    for py in range(2):
+        for px in range(2):
+            for ty in range(2):
+                for tx in range(2):
+                    out[py * 2 + px, :, :, ty, tx] = w[:, :, 3 - py - 2 * ty, 3 - px - 2 * tx].T
+    return out
+
+
 class Engine:
     """The backbone + heads of ACR as one precompiled CUDA launch plan.
 
@@ -98,12 +112,16 @@ class Engine:
     after the trunk, fed by an external (B,32,H/4,W/4) feature through ``run_heads``.
     ``weights`` re-uses the packed weight blob of another engine of the same dtype / flags (the blob does
     not depend on the batch size).
+    ``backbone``: "hrnet" (HRNet-W32, or the trunk ``widths`` names) or "resnet50" (netspec.build_acr_spec): the
+    ResNet-50 trunk runs on the tensor cores only (7x7 stem, max-pool, 1x1 stride-2 and transposed convs have no fp32
+    validation or CUDA-core form), so fp32 and ``debug_ref_conv`` raise AcrB200Error for it.
     """
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], batch: int, device, act_dtype=torch.bfloat16,
                  input_size: int = 512, debug_ref_conv: bool = False, reuse_memory: bool = True,
                  dry_run: bool = False, keep_extra=(), stem_on_tensor_cores: bool = True,
-                 head_only: bool = False, weights: Optional[torch.Tensor] = None, widths=None):
+                 head_only: bool = False, weights: Optional[torch.Tensor] = None, widths=None,
+                 backbone: str = "hrnet"):
         self.keep_extra = tuple(keep_extra)   # extra tensor names kept alive after the run (tests)
         self.dry_run = dry_run      # layout only (arena size, op list); used by CPU tests
         if not dry_run and not torch.cuda.is_available():
@@ -118,6 +136,10 @@ class Engine:
         self.f32 = act_dtype == torch.float32
         self.esz = 4 if self.f32 else 2
         self.npw = np.float32 if self.f32 else np.uint16      # numpy type of one packed weight
+        if backbone == "resnet50" and (self.f32 or debug_ref_conv):
+            raise L.AcrB200Error("Engine: the ResNet-50 trunk runs on the tensor cores only (no fp32 validation plan, "
+                                 "no debug_ref_conv): use act_dtype torch.bfloat16 or torch.float16")
+        self.backbone = backbone
         self.stem_on_tensor_cores = stem_on_tensor_cores and not self.f32
         self.head_only = head_only
         from .netspec import WIDTHS
@@ -126,7 +148,8 @@ class Engine:
         self.spec: NetSpec = build_acr_spec(input_size, merge_stems=os.environ.get("ACR_B200_MERGE_STEMS", "1") != "0",
                                             widths=tuple(widths) if widths else WIDTHS,
                                             fold_fuse=(os.environ.get("ACR_B200_FOLD_FUSE", "0") != "0"
-                                                       and act_dtype != torch.float32 and not debug_ref_conv))
+                                                       and act_dtype != torch.float32 and not debug_ref_conv),
+                                            backbone=backbone)
         self.input_size = input_size
         self.flops_per_image = conv_flops_per_image(self.spec)
         self.debug_ref_conv = debug_ref_conv or self.f32
@@ -172,6 +195,21 @@ class Engine:
         L.check(self.lib.acr_b200_pack_conv(p(w), p(cb), p(bn[0]), p(bn[1]), p(bn[2]), p(bn[3]), BN_EPS, cout, cin, k,
                                             cout_pad, cin_pad, self.dt, wp.ctypes.data, bias.ctypes.data),
                 "pack_conv " + wkey)
+        return blob.add(wp), blob.add(bias)
+
+    def _pack_deconv(self, sd, blob: _Blob, wkey: str, bnkey: str, cin_pad: int, cout_pad: int) -> Tuple[int, int]:
+        """ConvTranspose2d + BN -> [4 parities][cout_pad][4 taps][cin_pad] 16-bit (BN folded by pack_conv, parity by
+        parity) + fp32 bias[cout_pad] (csrc/conv_tc.cuh MODE_DECONV)."""
+        par = deconv_parity_weights(np.ascontiguousarray(sd[wkey + ".weight"], np.float32))
+        bn = [np.ascontiguousarray(sd[f"{bnkey}.{n}"], np.float32) for n in ("weight", "bias", "running_mean", "running_var")]
+        cout, cin = par.shape[1:3]
+        wp = np.zeros((4, cout_pad, 4, cin_pad), self.npw)
+        bias = np.zeros(cout_pad, np.float32)
+        for p in range(4):
+            w = np.ascontiguousarray(par[p])
+            L.check(self.lib.acr_b200_pack_conv(w.ctypes.data, None, *(b.ctypes.data for b in bn), BN_EPS, cout, cin, 2,
+                                                cout_pad, cin_pad, self.dt, wp[p].ctypes.data, bias.ctypes.data),
+                    "pack_conv " + wkey)
         return blob.add(wp), blob.add(bias)
 
     def _pack_raw(self, blob: _Blob, w: np.ndarray, cin_pad: int, cout_pad: int) -> int:
@@ -231,6 +269,16 @@ class Engine:
                 recs.append(dict(kind=L.OP_CONV_REF if self.debug_ref_conv else L.OP_CONV, out=op.out,
                                  ins=[op.ins[1]], aux=[bias_img[s]],
                                  attrs=dict(k=1, s=1, relu=False, residual=False, pow11=False, fold_side=s)))
+            elif op.kind == "stem" and op.attrs.get("k") == 7:
+                # ResNet conv1 7x7 s2 + bn1 + relu: the same shared-memory-operand GEMM with K = 147 taps + bias (160)
+                if not (_pow2(op.out.W // 16) and _pow2(op.out.H // 16)):
+                    raise L.AcrB200Error(f"Engine: the 7x7 stem needs power-of-two tile counts, input {self.input_size} "
+                                         "is not a power-of-two multiple of 512")
+                recs.append(dict(kind=L.OP_STEM_TC, out=op.out, ins=[op.ins[0]], attrs=dict(stem=op.attrs)))
+            elif op.kind == "maxpool":
+                recs.append(dict(kind=L.OP_MAXPOOL, out=op.out, ins=[op.ins[0]]))
+            elif op.kind == "deconv":
+                recs.append(dict(kind=L.OP_CONV, out=op.out, ins=[op.ins[0]], attrs=op.attrs))
             elif op.kind == "stem" and self.stem_on_tensor_cores and not self.debug_ref_conv \
                     and os.environ.get("ACR_B200_STEM_FUSED", "1") != "0" and _pow2(op.out.W // 16) and _pow2(op.out.H // 16):
                 # conv1 + bn1 + relu as ONE wgmma GEMM whose im2col operand is built in shared memory (csrc/stem_tc.cu)
@@ -347,7 +395,11 @@ class Engine:
                     o.shift[0] |= 16    # ACR_CONV_EXTRA: in_[1..] are further terms, nearest-upsampled by 2**shift[j]
                     for q, (_, sh) in enumerate(a["extra"]):
                         o.shift[1 + q] = sh
-                if "stem" in a:
+                if a.get("deconv"):
+                    o.cin_pad = _rup(x.C, 64)
+                    o.w_offset[0], o.w_offset[1] = self._pack_deconv(sd, blob, a["w"], a["bn"], o.cin_pad, o.cout_pad)
+                    o.shift[0] |= L.CONV_DECONV
+                elif "stem" in a:
                     # weights (64,3,3,3) OIHW -> (64, 32, 1, 1) with input channel (ky*3+kx)*3+ci; BN folded by pack_conv
                     w = f32(a["stem"]["w"] + ".weight")
                     w1 = np.zeros((64, 32, 1, 1), np.float32)
@@ -394,14 +446,19 @@ class Engine:
                     if a.get("pow11"):
                         o.shift[0] |= 2  # ACR_CONV_POW11_CH0
             elif r["kind"] == L.OP_STEM_TC:
-                # weights (64,3,3,3) OIHW -> (64, 32, 1, 1) with input channel (ky*3+kx)*3+ci; BN folded by pack_conv
+                # weights (64,3,k,k) OIHW -> (64, K, 1, 1) with input channel (ky*k+kx)*3+ci, K = 32 (3x3) or 160 (7x7: k = 7
+                # in the op); BN folded by pack_conv
                 w = f32(a["stem"]["w"] + ".weight")
-                w1 = np.zeros((64, 32, 1, 1), np.float32)
-                w1[:, :27, 0, 0] = w.transpose(0, 2, 3, 1).reshape(64, 27)
+                ks = w.shape[-1]
+                kch = 32 if ks == 3 else 160
+                w1 = np.zeros((64, kch, 1, 1), np.float32)
+                w1[:, :3 * ks * ks, 0, 0] = w.transpose(0, 2, 3, 1).reshape(64, 3 * ks * ks)
                 sd_stem = {"stem.weight": w1}
                 for nme in ("weight", "bias", "running_mean", "running_var"):
                     sd_stem[f"stembn.{nme}"] = f32(f"{a['stem']['bn']}.{nme}")
-                o.w_offset[0], o.w_offset[1] = self._pack_conv(sd_stem, blob, "stem", "stembn", False, 32, 64)
+                o.w_offset[0], o.w_offset[1] = self._pack_conv(sd_stem, blob, "stem", "stembn", False, kch, 64)
+                if ks == 7:
+                    o.k = 7
             elif r["kind"] == L.OP_STEM:
                 w = f32(a["w"] + ".weight")                                   # (64,3,3,3) OIHW
                 g_, b_, m_, v_ = (f32(f"{a['bn']}.{n}") for n in ("weight", "bias", "running_mean", "running_var"))

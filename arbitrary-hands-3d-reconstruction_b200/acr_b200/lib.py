@@ -15,6 +15,8 @@ LIB_PATH = os.environ.get("ACR_B200_LIB") or os.path.join(os.path.dirname(_HERE)
 
 OK = 0
 OP_STEM, OP_CONV, OP_FUSE, OP_BILINEAR2X, OP_COORD, OP_POOL, OP_PARTHEAD, OP_CONV_REF, OP_FINALCONV, OP_IM2COL_STEM, OP_STEM_TC = range(1, 12)
+OP_MAXPOOL = 12
+CONV_DECONV = 32      # ACR_CONV_DECONV flag bit (shift[0]) of a CONV op
 DT_BF16, DT_F16, DT_F32, DT_U8 = 0, 1, 2, 3
 
 

@@ -120,6 +120,16 @@ class NetSpec:
                                                    relu=relu, residual=False, pow11=False, merged=cout)))
         return slices
 
+    def deconv(self, x: Tensor, wkey: str, bnkey: str, cout: int, out: Optional[Tensor] = None) -> Tensor:
+        """nn.ConvTranspose2d(x.C, cout, 4, stride 2, padding 1, bias=False) + BN + ReLU: (C,H,W) -> (cout,2H,2W).  The
+        weight is registered in ConvTranspose2d's own layout (cin, cout, 4, 4)."""
+        self._reg(wkey + ".weight", (x.C, cout, 4, 4), "deconv_w")
+        self._reg_bn(bnkey, cout)
+        y = out if out is not None else self._t(cout, 2 * x.H, 2 * x.W, wkey.split(".")[-1])
+        self.ops.append(Op("deconv", y, [x], dict(w=wkey, bn=bnkey, k=4, s=2, relu=True, residual=False, pow11=False,
+                                                   deconv=True)))
+        return y
+
     def fuse(self, terms: List[Tuple[Tensor, int]], relu=True, out: Optional[Tensor] = None) -> Tensor:
         t0 = terms[0][0]
         H, W = t0.H << terms[0][1], t0.W << terms[0][1]
@@ -202,8 +212,42 @@ def _hr_module(g: NetSpec, prefix: str, xs: List[Tensor], multi_scale_output: bo
 WIDTHS_W48 = (48, 96, 192, 384)
 
 
+BACKBONES = ("hrnet", "resnet50")
+
+
+def _resnet_bottleneck(g: NetSpec, x: Tensor, p: str, planes: int, stride: int, down: bool) -> Tensor:
+    # acr/model.py:501-539 with the stride on conv2; registry order = construction order (conv1, bn1, conv2, bn2, conv3,
+    # bn3, then the downsample that _make_layer (:738-752) hands to the first block)
+    y = g.conv(x, p + ".conv1", p + ".bn1", planes, 1, relu=True)
+    y = g.conv(y, p + ".conv2", p + ".bn2", planes, 3, s=stride, relu=True)
+    out, op3 = g.conv(y, p + ".conv3", p + ".bn3", planes * 4, 1, relu=True, residual=x, defer=True)
+    if down:   # 1x1 stride-s conv + BN (padding 0: it reads input pixel (s*y, s*x))
+        op3.ins[1] = g.conv(x, p + ".downsample.0", p + ".downsample.1", planes * 4, 1, s=stride)
+    g.ops.append(op3)
+    return out
+
+
+def _resnet50_trunk(g: NetSpec, img: Tensor, S: int, feat: Tensor) -> None:
+    """ResNet-50 + three deconvs, ending in ``feat`` (32 channels at S/4)."""
+    g._reg("backbone.conv1.weight", (64, 3, 7, 7), "conv_w")
+    g._reg_bn("backbone.bn1", 64)
+    x = g._t(64, S // 2, S // 2, "stem7")
+    g.ops.append(Op("stem", x, [img], dict(w="backbone.conv1", bn="backbone.bn1", k=7)))
+    y = g._t(64, S // 4, S // 4, "maxpool")
+    g.ops.append(Op("maxpool", y, [x], {}))
+    x, cin = y, 64
+    for L, (planes, blocks, stride) in enumerate(((64, 3, 1), (128, 4, 2), (256, 6, 2), (512, 3, 2)), 1):
+        for i in range(blocks):
+            s = stride if i == 0 else 1
+            x = _resnet_bottleneck(g, x, f"backbone.layer{L}.{i}", planes, s, down=(i == 0 and (s != 1 or cin != planes * 4)))
+            cin = planes * 4
+    for j, cout in enumerate((256, 128, 32)):   # deconv_layers = [ConvT, BN, ReLU] x 3
+        x = g.deconv(x, f"backbone.deconv_layers.{3 * j}", f"backbone.deconv_layers.{3 * j + 1}", cout,
+                     out=feat if j == 2 else None)
+
+
 def build_acr_spec(input_size: int = 512, merge_stems: bool = True, widths: Tuple[int, ...] = WIDTHS,
-                   fold_fuse: bool = False) -> NetSpec:
+                   fold_fuse: bool = False, backbone: str = "hrnet") -> NetSpec:
     """Full ACR network for one image of ``input_size`` x ``input_size``.  ``merge_stems=False`` keeps the eight
     head stem convs as eight launches (A/B timing of the merged form).  ``fold_fuse``: the fuse sums of the coarser
     outputs (i >= 1) of every HighResolutionModule (acr/model.py:677-684) run in the epilogue of the stride-2 conv that
@@ -215,13 +259,40 @@ def build_acr_spec(input_size: int = 512, merge_stems: bool = True, widths: Tupl
     contains: /root/reference/acr/model.py:796-797, SURVEY F1/F2).  WIDTHS_W48 = (48, 96, 192, 384) is the HRNet-W48
     trunk BASELINE.json's configs[4] names: it has no reference implementation -- the same topology with wider
     branches, the heads reading a (widths[0] + 2)-channel map -- so its PARITY IS UNPINNED (no golden can exist); it is
-    measured for throughput and pinned op by op only against the oracle's per-op restatement."""
+    measured for throughput and pinned op by op only against the oracle's per-op restatement.
+
+    ``backbone="resnet50"``: the ResNet-50 trunk of BASELINE.json's configs 1-2.  The reference contains no ResNet trunk
+    (SURVEY F1/F2: ``--backbone`` is only a log tag there), so this spec FIXES one definition and its parity is
+    unpinned, like W48.  It is built from the reference's own blocks: conv1 7x7 s2 p3 3->64 (no bias) + bn1 + ReLU on
+    x/255*2-1 (as acr/model.py:832), MaxPool 3x3 s2 p1, then _make_layer(Bottleneck, 64/128/256/512, 3/4/6/3, stride
+    1/2/2/2) (:501-539, :738-752: stride on the 3x3 conv2, 1x1 stride-s downsample + BN whenever the stride or width
+    changes) -> 2048 channels at S/32, then 3 x [ConvTranspose2d k4 s2 p1 (no bias), BN, ReLU] with widths 256, 128, 32
+    (``backbone.deconv_layers.{0,1,3,4,6,7}``) -> 32 channels at S/4.  The trunk so ends in the same contract as
+    HigherResolutionNet (backbone_channels = 32, :697): SegmNet (:395 hard-codes 32 input channels), the coord concat,
+    both final-layer stacks and the part branch are the reference's own network, and every non-trunk key keeps the W32
+    model's name and shape, so the heads of a real checkpoint load unchanged.  The input size must be a multiple of
+    512: layer4 (S/32) runs on whole 16x16 tiles."""
+    if backbone not in BACKBONES:
+        raise ValueError(f"backbone must be one of {BACKBONES}, got {backbone!r}")
     g = NetSpec()
-    g.widths = tuple(widths)
-    W0, W1, W2, W3 = g.widths
+    g.backbone = backbone
     S = input_size
     img = Tensor("image", 3, S, S, "u8")
     g.tensors[img.name] = img
+    F = S // 4
+    if backbone == "resnet50":
+        if S % 512:
+            raise ValueError(f"the ResNet-50 trunk needs an input size that is a multiple of 512 (layer4 runs at S/32 on whole "
+                             f"16x16 tiles), got {S}")
+        g.widths = (32,)
+        xcat = g._t(34, F, F, "xcat")
+        feat = Tensor("feat32", 32, F, F, "act", base=xcat, c_off=0)
+        g.tensors[feat.name] = feat
+        _resnet50_trunk(g, img, S, feat)
+        _heads(g, xcat, feat, merge_stems)
+        return g
+    g.widths = tuple(widths)
+    W0, W1, W2, W3 = g.widths
 
     # ---- stem (acr/model.py:831-839): x/255*2-1, conv3x3 s2 + BN + ReLU, twice
     g._reg("backbone.conv1.weight", (64, 3, 3, 3), "conv_w")
@@ -247,7 +318,6 @@ def build_acr_spec(input_size: int = 512, merge_stems: bool = True, widths: Tupl
     # ---- transition3 + stage4 (3 modules, 4 branches; last keeps only branch 0)
     xs.append(g.conv(xs[-1], "backbone.transition3.3.0.0", "backbone.transition3.3.0.1", W3, 3, s=2, relu=True))
     # the backbone output lands in channels [0:32) of the 34-channel coord-concat buffer
-    F = S // 4
     xcat = g._t(W0 + 2, F, F, "xcat")
     feat = Tensor("feat32", W0, F, F, "act", base=xcat, c_off=0)   # ("feat32": the name, not the width)
     g.tensors[feat.name] = feat
@@ -256,6 +326,14 @@ def build_acr_spec(input_size: int = 512, merge_stems: bool = True, widths: Tupl
         xs = _hr_module(g, f"backbone.stage4.{m}", xs, not last, out0=feat if last else None, WIDTHS=g.widths, fold_fuse=fold_fuse)
     x = xs[0]
     assert x is feat
+    _heads(g, xcat, feat, merge_stems)
+    return g
+
+
+def _heads(g: NetSpec, xcat: Tensor, feat: Tensor, merge_stems: bool) -> None:
+    """Everything after the trunk (acr/model.py:47-65 head_forward), reading the trunk's feature ``feat`` = channels
+    [0, W0) of the (W0 + 2)-channel coord-concat buffer ``xcat``."""
+    W0, F = feat.C, feat.H
     # coord channels 32,33 are constants written once (acr/model.py:52, 340-369)
     g.ops.append(Op("coordcat", xcat, [feat], {}))
 
@@ -336,19 +414,26 @@ def build_acr_spec(input_size: int = 512, merge_stems: bool = True, widths: Tupl
     g._reg_bn("segmentation_layers.1.1", 256)
     g._reg("segmentation_layers.2.0.weight", (33, 256, 1, 1), "conv_w")
     g._reg("segmentation_layers.2.0.bias", (33,), "conv_b")
-    return g
+
+
+def op_flops(op: Op) -> float:
+    """2*MAC count of one conv-like op per image (0 for the others).  A transposed conv counts its LIVE taps only: every
+    output pixel of the k4 s2 p1 form sees 2x2 of the 16 taps."""
+    if op.kind == "conv":
+        x, y = op.ins[0], op.out
+        return 2.0 * y.H * y.W * y.C * x.C * op.attrs["k"] ** 2
+    if op.kind == "deconv":
+        x, y = op.ins[0], op.out
+        return 2.0 * y.H * y.W * y.C * x.C * 4
+    if op.kind == "stem":
+        return 2.0 * op.out.H * op.out.W * 64 * 3 * op.attrs.get("k", 3) ** 2
+    return 0.0
 
 
 def conv_flops_per_image(spec: NetSpec) -> float:
-    """2*MAC count of every executed Conv2d/Linear + the two pooling matmuls
+    """2*MAC count of every executed Conv2d/ConvTranspose2d/Linear + the two pooling matmuls
     (SURVEY.md section 8d: 102.12 GFLOP/img for HRNet-W32 at 512x512)."""
-    fl = 0.0
-    for op in spec.ops:
-        if op.kind == "conv":
-            x, y = op.ins[0], op.out
-            fl += 2.0 * y.H * y.W * y.C * x.C * op.attrs["k"] ** 2
-        elif op.kind == "stem":
-            fl += 2.0 * op.out.H * op.out.W * 64 * 27
+    fl = sum(op_flops(op) for op in spec.ops)
     F = spec.tensors["feat32"].H
     fl += 2.0 * F * F * 64 * 256               # cam_shape_layers[1] 1x1 conv 256->64
     fl += 2 * 2.0 * F * F * 109 * 218 / 4      # contact_layers[4,5] at (F/2)^2

@@ -28,7 +28,7 @@ MANO_PARENTS = [-1, 0, 1, 2, 0, 4, 5, 0, 7, 8, 0, 10, 11, 0, 13, 14]
 def synth_state_dict(seed: int = 0, spec: Optional[NetSpec] = None,
                      bn_stats: Optional[Dict[str, np.ndarray]] = None,
                      center_bias: float = 1.0) -> "OrderedDict[str, torch.Tensor]":
-    """Random-init weights with the reference's 2067 state-dict keys.
+    """Random-init weights with the reference's 2067 state-dict keys (or those of ``spec``: any trunk).
 
     * conv / linear weights: N(0, gain^2 * 2/fan_in); the last BN of each residual
       block and the fuse-layer BNs get a small gamma so activations stay O(1)
@@ -45,6 +45,8 @@ def synth_state_dict(seed: int = 0, spec: Optional[NetSpec] = None,
         if kind == "conv_w":
             fan_in = shape[1] * shape[2] * shape[3]
             w = torch.randn(shape, generator=g) * math.sqrt(2.0 / fan_in)
+        elif kind == "deconv_w":   # ConvTranspose2d (cin, cout, 4, 4), k4 s2: every output pixel sees cin x 2 x 2 live taps
+            w = torch.randn(shape, generator=g) * math.sqrt(2.0 / (shape[0] * 4))
         elif kind == "lin_w":
             w = torch.randn(shape, generator=g) * math.sqrt(1.0 / shape[1])
         elif kind == "lc_w":

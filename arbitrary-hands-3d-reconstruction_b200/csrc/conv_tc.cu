@@ -58,10 +58,14 @@ static bool p1_enabled() {
 
 int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   ACR_CHECK_ARG(a.out.H % TILE_Y == 0 && a.out.W % TILE_X == 0, "conv_tc: output %dx%d is not a multiple of the 16x16 super-tile", a.out.H, a.out.W);
-  ACR_CHECK_ARG(a.in.pix_stride % 8 == 0 && a.cin_pad % 16 == 0 && a.cout_pad % 16 == 0 && a.cout_pad <= 1024,
+  ACR_CHECK_ARG(a.in.pix_stride % 8 == 0 && a.cin_pad % 16 == 0 && a.cout_pad % 16 == 0 && a.cout_pad <= 2048 && a.cin_pad <= 2048,
                 "conv_tc: channel alignment");
   ACR_CHECK_ARG(a.in.dtype == act_dtype, "conv_tc: input dtype mismatch");
-  ACR_CHECK_ARG(!(a.k == 1 && a.stride != 1), "conv_tc: 1x1 stride-2 unsupported");
+  ACR_CHECK_ARG(!a.deconv || (a.k == 4 && a.stride == 2 && a.cin_pad % 64 == 0 && !a.has_res && a.n_ext == 0 && !a.xpair &&
+                              !a.s2x && !a.bias_per_image && !a.pow11_ch0 && a.out.H == 2 * a.in.H && a.out.W == 2 * a.in.W &&
+                              a.in.H % TILE_Y == 0 && a.in.W % TILE_X == 0),
+                "conv_tc: the transposed conv is k4 s2 p1 over whole 16x16 input tiles, 64-channel K chunks, no residual");
+  ACR_CHECK_ARG(a.deconv || a.k == 1 || a.k == 3, "conv_tc: kernel size %d", a.k);
   ACR_CHECK_ARG(!a.xpair || (a.k == 3 && a.stride == 1 && a.cin_pad == 64 && a.cout_pad == 64 && a.in.pix_stride >= 64),
                 "conv_tc: the x-paired form is a 3x3 stride-1 64->64 conv");
   ACR_CHECK_ARG(!a.s2x || (a.k == 3 && a.stride == 2 && a.cin_pad == 64 && a.in.pix_stride == 64 && a.in.C == 64 && !a.xpair &&
@@ -77,8 +81,9 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   // subsets within a tap row, which ptxas serialises for lack of registers
   p.patch1 = (p.patch_mode && ck == 64 && !a.xpair && p1_enabled()) ? 1 : 0;
   p.s2x = a.s2x ? 1 : 0;
-  const cuuint32_t box_rows = p.s2x ? TILE_Y + 1 : (p.patch_mode ? TILE_Y + 2 : TILE_Y);
-  const cuuint32_t box_cols = (p.patch1 || p.s2x) ? P1_PITCH : TILE_X;
+  p.deconv = a.deconv ? 1 : 0;
+  const cuuint32_t box_rows = p.s2x ? TILE_Y + 1 : ((p.patch_mode || p.deconv) ? TILE_Y + 2 : TILE_Y);
+  const cuuint32_t box_cols = (p.patch1 || p.s2x || p.deconv) ? P1_PITCH : TILE_X;
   const cuuint64_t esz = 2;
   const cuuint64_t dim0 = (cuuint64_t)(a.cin_pad < a.in.pix_stride ? a.cin_pad : a.in.pix_stride);
   int rc = ACR_B200_OK;
@@ -92,7 +97,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
       rc = encode(&p.tmA[v], act_dtype, 4, ptr, dims, str, box, ck);
     }
     for (int v = 2; v < 4 && !rc; ++v) p.tmA[v] = p.tmA[0];
-  } else if (a.stride == 1) {
+  } else if (a.stride == 1 || a.deconv) {   // (the transposed conv reads its input at stride 1)
     cuuint64_t dims[4] = {dim0, (cuuint64_t)a.in.W, (cuuint64_t)a.in.H, (cuuint64_t)a.batch};
     cuuint64_t str[3] = {(cuuint64_t)a.in.pix_stride * esz, (cuuint64_t)a.in.W * a.in.pix_stride * esz,
                          (cuuint64_t)a.in.H * a.in.W * a.in.pix_stride * esz};
@@ -100,6 +105,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
     rc = encode(&p.tmA[0], act_dtype, 4, a.in.ptr, dims, str, box, ck);
     for (int v = 1; v < 4 && !rc; ++v) p.tmA[v] = p.tmA[0];
   } else {
+    // four parity views (even / odd rows x columns); a 1x1 stride-2 conv (padding 0) reads view 0 at offset 0 only
     for (int v = 0; v < 4 && !rc; ++v) {
       const int py = v >> 1, px = v & 1;
       const char* ptr = static_cast<const char*>(a.in.ptr) + ((size_t)py * a.in.W + px) * a.in.pix_stride * esz;
@@ -122,7 +128,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
     p.ext[e] = a.ext[e].ptr; p.ext_shift[e] = a.ext_shift[e]; p.ext_stride[e] = a.ext[e].pix_stride;
     p.ext_W[e] = a.ext[e].W; p.ext_H[e] = a.ext[e].H;
   }
-  p.tma_out = (tma_out_enabled() && a.out.dtype != ACR_DT_F32 && nsub % 64 == 0 && (uintptr_t)a.out.ptr % 16 == 0 &&
+  p.tma_out = (tma_out_enabled() && !a.deconv && a.out.dtype != ACR_DT_F32 && nsub % 64 == 0 && (uintptr_t)a.out.ptr % 16 == 0 &&
                a.out.pix_stride % 8 == 0) ? 1 : 0;
   if (p.tma_out) {
     cuuint64_t dims[4] = {(cuuint64_t)a.cout_pad, (cuuint64_t)a.out.W, (cuuint64_t)a.out.H, (cuuint64_t)a.batch};
@@ -134,30 +140,34 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   }
   p.stage_out_bytes = p.tma_out ? 4u * 8192u : 0u;
   p.bias = a.bias; p.res = a.has_res ? a.res.ptr : nullptr; p.out = a.out.ptr;
-  p.taps = a.k * a.k; p.ksz = a.k; p.stride = a.stride; p.cchunks = a.cin_pad / ck; p.cin_pad = a.cin_pad;
+  p.taps = a.deconv ? 4 : a.k * a.k; p.ksz = a.k; p.stride = a.stride; p.cchunks = a.cin_pad / ck; p.cin_pad = a.cin_pad;
   p.npad = a.cout_pad; p.nsplit = nsplit; p.nsub = nsub;
   pl->nt = nsub <= 64 ? 64 : 128;   // MMA width (a compile-time kernel parameter): the columns past nsub are not stored
   p.relu = a.relu; p.has_res = a.has_res; p.out_f32 = a.out.dtype == ACR_DT_F32;
   p.bias_per_image = a.bias_per_image; p.pow11_ch0 = a.pow11_ch0;
   p.xpair = a.xpair;
-  p.tiles_x = a.out.W / TILE_X; p.tiles_per_img = p.tiles_x * (a.out.H / TILE_Y);
+  // super-tiles cover the output grid, or the input grid of a transposed conv (each input tile feeds 4 output parities)
+  const int grid_h = a.deconv ? a.in.H : a.out.H, grid_w = a.deconv ? a.in.W : a.out.W;
+  p.tiles_x = grid_w / TILE_X; p.tiles_per_img = p.tiles_x * (grid_h / TILE_Y);
   p.total_tiles = p.tiles_per_img * a.batch;
+  const int npar = a.deconv ? 4 : 1;
   p.Ho = a.out.H; p.Wo = a.out.W; p.out_stride = a.out.pix_stride;
   p.res_stride = a.has_res ? a.res.pix_stride : 0;
   // shared-memory plan
   p.a_stage_bytes = (uint32_t)(box_rows * box_cols) * ck * 2;
   // resident weights: every output channel of a (tap, chunk) in one box (<= 256 rows); streamed: one virtual tile's rows
-  const size_t b_total = a.cout_pad <= 256 ? (size_t)p.taps * p.cchunks * a.cout_pad * ck * 2 : (size_t)1 << 40;
+  // (the transposed conv always streams: its [4 parities][cout_pad] rows are read one virtual tile at a time)
+  const size_t b_total = (a.cout_pad <= 256 && !a.deconv) ?(size_t)p.taps * p.cchunks * a.cout_pad * ck * 2 : (size_t)1 << 40;
   p.bias_bytes = (uint32_t)(((size_t)a.cout_pad * 4 + 1023) & ~(size_t)1023);
   const size_t fixed = 1024 /*alignment slack*/ + p.bias_bytes + 512 /*barriers*/ + p.stage_out_bytes;
-  const int nA = p.s2x ? 2 : (p.patch1 ? p.cchunks : (p.patch_mode ? p.cchunks * 3 : p.taps * p.cchunks));
+  const int nA = p.deconv ? p.cchunks : (p.s2x ? 2 : (p.patch1 ? p.cchunks : (p.patch_mode ? p.cchunks * 3 : p.taps * p.cchunks)));
   // stages that must fit next to resident weights: a tile's worth of kx patches (3) for 3x3 stride-1 convs, 2 otherwise
   const size_t min_a = (size_t)((p.patch_mode && !p.patch1) ? 3 : 2) * (size_t)p.a_stage_bytes;
   p.b_resident = (b_total + min_a + fixed <= (size_t)SMEM_BUDGET) ? 1 : 0;
   p.b_block_bytes = (uint32_t)(p.b_resident ? a.cout_pad : pl->nt) * ck * 2;
   {
-    const int taps = a.k * a.k;
-    cuuint64_t dims[2] = {(cuuint64_t)taps * a.cin_pad, (cuuint64_t)a.cout_pad};
+    const int taps = p.taps;
+    cuuint64_t dims[2] = {(cuuint64_t)taps * a.cin_pad, (cuuint64_t)npar * a.cout_pad};
     cuuint64_t str[1] = {(cuuint64_t)taps * a.cin_pad * esz};
     cuuint32_t box[2] = {(cuuint32_t)ck, (cuuint32_t)(p.b_resident ? a.cout_pad : pl->nt)};   // rows past cout_pad: zero fill
     rc = encode(&p.tmB, act_dtype, 2, a.w, dims, str, box, ck);
@@ -177,14 +187,15 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   int SA = (int)(((size_t)SMEM_BUDGET - fixed - p.b_region_bytes) / p.a_stage_bytes);
   if (SA > 8) SA = 8;
   if (SA > 2 * nA && !p.patch1) SA = 2 * nA;  // no point in more stages than two super-tiles' worth of loads
-  if ((p.patch1 || p.s2x) && SA > 4) SA = 4;
+  if ((p.patch1 || p.s2x || p.deconv) && SA > 4) SA = 4;
   if (SA < 2) { set_error("conv_tc: shared memory plan does not fit (cout_pad %d, ck %d)", a.cout_pad, ck); delete pl; return ACR_B200_EINVAL; }
   p.SA = SA;
   // ping-pong teams need every A load of a tile in the ring at once (conv_tc_kernel); the four-view stride-2 convs
   // (9 loads per channel chunk) and the 16-channel-chunk patch convs with several chunks stay in lockstep
   p.pingpong = (p.b_resident && nA <= SA) ? 1 : 0;
   pl->smem = fixed + p.b_region_bytes + (size_t)SA * p.a_stage_bytes;
-  pl->grid = p.total_tiles * nsplit < num_sms() ? p.total_tiles * nsplit : num_sms();
+  const int nvt = p.total_tiles * nsplit * npar;
+  pl->grid = nvt < num_sms() ? nvt : num_sms();
   *out = pl;
   return ACR_B200_OK;
 }

@@ -21,6 +21,8 @@
 //     the whole kernel when they fit (all 32/64-channel layers), otherwise streamed through their own mbarrier ring.
 //   * Both land in shared memory in the canonical K-major swizzled layout (128B / 64B / 32B swizzle for CK = 64 / 32 / 16)
 //     that wgmma descriptors address directly.
+//   * 1x1 stride-2 convs read parity view 0 at offset 0 (padding 0); transposed convs (MODE_DECONV) are four 2x2 convs
+//     on the input grid, one per output parity.
 //   * Persistent CTAs (one per SM): warps 0..15 = the four consumer warpgroups (wgmma issue, then the epilogue straight
 //     from the accumulator registers: +bias (+residual) (+extra terms) (ReLU) -> 16-bit / fp32 NHWC); warps 16..19 = the
 //     producer warpgroup, whose first warp issues the TMA loads and runs ahead into the next tile's operands.  The producer
@@ -152,6 +154,7 @@ struct ConvTcParams {
   int pingpong;   // resident weights and a tile's A loads fit in the ring: the consumer teams alternate (see the kernel)
   int patch1;   // MODE_P1: ONE 24-wide haloed box per channel chunk, kx shifts = unaligned descriptor starts
   int s2x;      // MODE_S2X: 3x3 stride-2 conv of a dense 32-channel tensor read as x-pairs: two row-parity boxes per tile
+  int deconv;   // MODE_DECONV: transposed conv k4 s2 p1; tiles_x / tiles_per_img count INPUT super-tiles, Ho / Wo the output
   uint32_t a_stage_bytes, b_block_bytes, b_region_bytes;
   int tiles_x, tiles_per_img, total_tiles, Ho, Wo, out_stride, res_stride;
 };
@@ -186,14 +189,24 @@ constexpr int P1_PITCH = 24;   // pixels per image row of the single box
 // 0/1 = an unaligned start, K half 0/1 = k-steps {0,1} or {2,3}).  The packed weights carry the 32 input channels
 // of tap (ky,kx) at K offset 32*(kx != 1) (engine._pack_conv(s2x=True)).
 constexpr int MODE_S2X = 32;
+// MODE_DECONV (CK = 64, streamed weights, lockstep): ConvTranspose2d kernel 4 stride 2 padding 1.  Output pixel
+// (2m+py, 2n+px) is a 2x2 conv of the input at offsets {py-1, py} x {px-1, px}, so every output parity is an ordinary
+// conv on the INPUT grid: the super-tile is 16x16 input pixels, read as the MODE_P1 haloed box {64, 24, 18} from
+// (x0-1, y0-1), and parity (py,px) issues only its 4 live taps, tap (ty,tx) = descriptor start (py+ty) rows and (px+tx)
+// pixels into the box.  Parity x N split are virtual tiles (parity-major within a super-tile); the weights are
+// [4 parities][cout_pad][4 taps][cin_pad], so parity p streams rows p * cout_pad + n_off.  The epilogue stores at
+// stride 2: pixel (2 oy + py, 2 ox + px) of the output.
+constexpr int MODE_DECONV = 64;
 
 template <int CK, typename T, int MODE, int NT>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ ConvTcParams P) {
   using Cfg = SwizzleCfg<CK>;
   constexpr bool PATCH = (MODE & MODE_PATCH) != 0, RESIDENT = (MODE & MODE_RESIDENT) != 0, XPAIR = (MODE & MODE_XPAIR) != 0;
-  constexpr bool P1 = (MODE & MODE_P1) != 0, S2X = (MODE & MODE_S2X) != 0;
+  constexpr bool P1 = (MODE & MODE_P1) != 0, S2X = (MODE & MODE_S2X) != 0, DECONV = (MODE & MODE_DECONV) != 0;
+  constexpr int NPAR = DECONV ? 4 : 1;   // virtual tiles per (super-tile, N split)
   static_assert(!P1 || (PATCH && CK == 64 && !XPAIR), "the single-box form exists for CK = 64 patch convs (not x-paired)");
   static_assert(!S2X || (!PATCH && !P1 && !XPAIR && CK == 64), "the x-paired stride-2 form is a CK = 64 mode of its own");
+  static_assert(!DECONV || (MODE == MODE_DECONV && CK == 64), "the transposed conv is a CK = 64 streamed-weight mode of its own");
   static_assert((NT == 64 || NT == 128) && (!XPAIR || NT == 64), "MMA width: 64 or 128 columns (x-paired convs: 64)");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -214,8 +227,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   float* s_bias = reinterpret_cast<float*>(smem_raw + (bias_base - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int nA = P.s2x ? 2 : (P.patch1 ? P.cchunks : (P.patch_mode ? P.cchunks * 3 : P.taps * P.cchunks));  // A loads per super-tile
-  const int nsub_taps = P.patch1 ? 9 : (P.patch_mode ? 3 : 1);                                 // taps served by one A load
+  const int nA = DECONV ? P.cchunks : (P.s2x ? 2 : (P.patch1 ? P.cchunks : (P.patch_mode ? P.cchunks * 3 : P.taps * P.cchunks)));  // A loads per super-tile
+  const int nsub_taps = DECONV ? 4 : (P.patch1 ? 9 : (P.patch_mode ? 3 : 1));                  // taps served by one A load
 
   if (threadIdx.x == 0) {
     // a stage is free again once every consumer warp has seen the wgmmas that read it complete
@@ -250,14 +263,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     pdl_wait();   // weights are constants; the activations below are the previous kernel's output
     int sa = 0, sb = 0;
     uint32_t pha = 0, phb = 0;
-    for (int vt = blockIdx.x; vt < P.total_tiles * P.nsplit; vt += gridDim.x) {
-      const int tile = vt / P.nsplit, n_off = (vt - tile * P.nsplit) * P.nsub;
+    for (int vt = blockIdx.x; vt < P.total_tiles * P.nsplit * NPAR; vt += gridDim.x) {
+      const int tile = vt / (P.nsplit * NPAR), vr = vt - tile * (P.nsplit * NPAR);
+      const int par = DECONV ? vr / P.nsplit : 0;
+      const int n_off = (vr - par * P.nsplit) * P.nsub;
+      const int b_row = DECONV ? par * P.npad + n_off : n_off;   // first weight row of this virtual tile
       const int n = tile / P.tiles_per_img, rem = tile % P.tiles_per_img;
       const int y0 = (rem / P.tiles_x) * TILE_Y, x0 = (rem % P.tiles_x) * TILE_X;
       for (int a = 0; a < nA; ++a) {
         int cc, view = 0, dy = 0, dx = 0, tap0;
         int nsub_a = nsub_taps;
-        if (P.s2x) {                  // a = row parity: even rows from y0 (taps ky=1), odd rows from y0-1 (ky=0,2)
+        if (DECONV) {                 // one 18x24 box per channel chunk, as MODE_P1; the parity picks taps inside it
+          cc = a; dy = -1; dx = -1; tap0 = 0;
+        } else if (P.s2x) {                // a = row parity: even rows from y0 (taps ky=1), odd rows from y0-1 (ky=0,2)
           cc = 0; view = a; dy = a ? -1 : 0; dx = -1; tap0 = 0; nsub_a = a ? 6 : 3;
         } else if (P.patch1) {        // one 18x24 box per channel chunk: rows y0-1 .. y0+16, columns x0-1 .. x0+22
           cc = a; dy = -1; dx = -1; tap0 = 0;
@@ -287,12 +305,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
           for (int sub = 0; sub < nsub_a; ++sub) {
             // weight block order = the consumers' tap order (single box: ky-major, kx 1,0,2 for x-paired convs;
             // stride-2 pairs: ky=1 with the even-row box, then ky=0 and ky=2 with the odd-row box)
-            const int tap = P.s2x ? (a == 0 ? 3 + sub : (sub < 3 ? sub : 3 + sub))
+            // (transposed conv: the 4 taps (ty,tx) of this parity, row-major)
+            const int tap = DECONV ? sub : P.s2x ? (a == 0 ? 3 + sub : (sub < 3 ? sub : 3 + sub))
                                   : (P.patch1 ? (sub / 3) * 3 + patch_kx(sub % 3, P.xpair) : (P.patch_mode ? sub * 3 + tap0 : tap0));
             mbar_wait_parity(emptyB(sb), phb ^ 1u);
             if (elect_one_sync()) {
               mbar_expect_tx(fullB(sb), P.b_block_bytes);
-              tma_load_2d(b_base + (uint32_t)sb * P.b_block_bytes, &P.tmB, fullB(sb), tap * P.cin_pad + cc * CK, n_off);
+              tma_load_2d(b_base + (uint32_t)sb * P.b_block_bytes, &P.tmB, fullB(sb), tap * P.cin_pad + cc * CK, b_row);
             }
             __syncwarp();
             if (++sb == SB) { sb = 0; phb ^= 1u; }
@@ -327,7 +346,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   const int h = wg & 1, rg = wg >> 1;           // half (left / right 8 columns), row group (image rows 0..7 / 8..15)
   if (RESIDENT) mbar_wait_parity(bres_bar, 0);
   pdl_wait();   // residual / extra-term / per-image bias reads and every output write wait for the previous kernel
-  constexpr uint32_t pitch16 = ((P1 || S2X) ? P1_PITCH * Cfg::kRowBytes : Cfg::kSBO_A) >> 4;   // image row pitch of the A box
+  constexpr uint32_t pitch16 = ((P1 || S2X || DECONV) ? P1_PITCH * Cfg::kRowBytes : Cfg::kSBO_A) >> 4;   // image row pitch of the A box
   const uint32_t hi_a = pitch16 | (Cfg::kSwizzle << 30);          // SBO = next image row (= next 8-pixel core-matrix group)
   const uint32_t hi_b = (Cfg::kAtom >> 4) | (Cfg::kSwizzle << 30);
   const uint32_t lo_flags = 1u << 16;                              // LBO (unused by swizzled K-major operands)
@@ -382,14 +401,31 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   int sa = 0, sb = 0;
   uint32_t pha = 0, phb = 0;
   uint32_t xa_bar[3];   // x-paired form: the three A stages of the tile, released once its MMAs completed
-  const int nvt = P.total_tiles * P.nsplit;
+  const int nvt = P.total_tiles * P.nsplit * NPAR;
   if (pingpong && rg == 1) named_bar_arrive_if(TEAM_BAR, 512, 1u);
   for (int vt = blockIdx.x; vt < nvt; vt += gridDim.x) {
     if (pingpong) named_bar_sync(TEAM_BAR + rg, 512);
     scale = 0;
     // resident weights hold all N rows: this virtual tile multiplies rows [n_off, n_off + NT)
     const uint32_t b_lo_base = b_lo_base0 + (RESIDENT ? (uint32_t)((vt % P.nsplit) * nsub) * (Cfg::kRowBytes >> 4) : 0u);
-    if (S2X) {
+    if (DECONV) {
+      // one A stage per channel chunk; parity (py,px) reads taps (ty,tx) at (py + ty) rows, (px + tx) pixels into it
+      const int par = (vt / P.nsplit) & 3;
+      const uint32_t a_par = a_lo_base + (uint32_t)(par >> 1) * pitch16 + (uint32_t)(par & 1) * (Cfg::kRowBytes >> 4);
+      for (int cc = 0; cc < cchunks; ++cc) {
+        mbar_wait_parity(fullA(sa), pha);
+        const uint32_t a_lo = a_par + (uint32_t)sa * a_stage16;
+#pragma unroll
+        for (int t = 0; t < 4; ++t) {
+          mbar_wait_parity(fullB(sb), phb);
+          wgmma_fence();
+          issue(a_lo + (uint32_t)(t >> 1) * pitch16 + (uint32_t)(t & 1) * (Cfg::kRowBytes >> 4), b_lo_base + (uint32_t)sb * b_block16, 1);
+          group_done(t == 3 ? emptyA(sa) : dummy_bar, emptyB(sb));
+          if (++sb == SB) { sb = 0; phb ^= 1u; }
+        }
+        if (++sa == SA) { sa = 0; pha ^= 1u; }
+      }
+    } else if (S2X) {
       // two A stages per tile (even-row box, odd-row box); tap (ky,kx): row offset (ky == 2), pair-column offset
       // (kx != 0), K half (kx != 1) -> k-steps {0,1} or {2,3} of the 64-wide row, same k-steps of the weight block
 #pragma unroll
@@ -510,7 +546,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 
     // ---------------------------------------------------------------- epilogue, straight from the register fragment
     // thread: pixels (image row 2 wq + r2 of this warpgroup's 8, column lane / 4), channels 8 j + 2 (lane % 4) + {0, 1}
-    const int tile = vt / P.nsplit, n_off = (vt - tile * P.nsplit) * nsub;
+    // (transposed conv: oy / ox below are input-grid coordinates, stored at output pixel (2 oy + py, 2 ox + px))
+    const int tile = vt / (P.nsplit * NPAR), vr = vt - tile * (P.nsplit * NPAR);
+    const int par = DECONV ? vr / P.nsplit : 0;
+    const int n_off = (vr - par * P.nsplit) * nsub;
     const int n = tile / P.tiles_per_img, rem = tile % P.tiles_per_img;
     const int oy0 = (rem / P.tiles_x) * TILE_Y + rg * 8 + 2 * wq, ox = (rem % P.tiles_x) * TILE_X + h * HALF_X + (lane >> 2);
     const int cq = 2 * (lane & 3);
@@ -529,7 +568,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
       for (int r2 = 0; r2 < 2; ++r2) {
         const int oy = oy0 + r2;
-        const size_t pix = ((size_t)n * P.Ho + oy) * P.Wo + ox;
+        const size_t pix = DECONV ? ((size_t)n * P.Ho + 2 * oy + (par >> 1)) * P.Wo + 2 * ox + (par & 1)
+                                  : ((size_t)n * P.Ho + oy) * P.Wo + ox;
         const T* resp = P.has_res ? reinterpret_cast<const T*>(P.res) + pix * P.res_stride + n_off : nullptr;
         const uint32_t srow = stage_wg + (uint32_t)(16 * wq + (lane >> 2) + 8 * r2) * 128u;   // slab row = pixel (row-major 8 x 8)
 #pragma unroll
@@ -617,6 +657,7 @@ template <int CK, typename T>
 static int launch_mode(const ConvTcPlan* pl, cudaStream_t st) {
   const int mode = (pl->p.patch_mode ? MODE_PATCH : 0) | (pl->p.b_resident ? MODE_RESIDENT : 0);
   if constexpr (CK == 64) {
+    if (pl->p.deconv) return launch_inst<64, T, MODE_DECONV>(pl, st);
     if (pl->p.s2x)
       return pl->p.b_resident ? launch_inst<64, T, MODE_RESIDENT | MODE_S2X>(pl, st) : launch_inst<64, T, MODE_S2X>(pl, st);
     if (pl->p.patch1)

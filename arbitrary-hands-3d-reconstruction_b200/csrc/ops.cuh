@@ -19,6 +19,7 @@ struct ConvArgs {
   TensorRef ext[3];        // ACR_CONV_EXTRA: up to three more terms added before the activation (HRNet fuse sums folded into
   int n_ext, ext_shift[3]; // the producing conv): term e is read at pixel (oy >> shift, ox >> shift) = nearest upsampling
   int s2x;                 // ACR_CONV_S2X: 3x3 stride-2 conv of a dense 32-channel tensor given as its x-paired view (H, W/2, 64)
+  int deconv;              // ACR_CONV_DECONV: ConvTranspose2d k4 s2 p1, weights [4 parities][cout_pad][4 taps][cin_pad]
 };
 
 struct FuseArgs {
@@ -31,9 +32,11 @@ int launch_stem(const TensorRef& img, const TensorRef& out, const float* w, cons
                 int act_dtype, cudaStream_t st);
 int launch_im2col_stem(const TensorRef& img, const TensorRef& out, int batch, int act_dtype, cudaStream_t st);
 // stem conv on the tensor cores with the A operand built in shared memory from the uint8 frame (stem_tc.cu): w = packed
-// [64][32] 16-bit (tap-major K, BN folded), bias fp32 [64]
+// [64][32] 16-bit (tap-major K, BN folded), bias fp32 [64]; ks = 7: the 7x7 stride-2 padding-3 stem, w = packed [64][160]
 int launch_stem_tc(const TensorRef& img, const TensorRef& out, const void* w, const float* bias, int batch, int act_dtype,
-                   cudaStream_t st);
+                   int ks, cudaStream_t st);
+// 3x3 stride-2 padding-1 max-pool on 16-bit NHWC (maxpool.cu)
+int launch_maxpool(const TensorRef& in, const TensorRef& out, int batch, int act_dtype, cudaStream_t st);
 int launch_conv_ref(const ConvArgs& a, int act_dtype, cudaStream_t st);
 int launch_fuse(const FuseArgs& a, int act_dtype, cudaStream_t st);
 int launch_bilinear2x(const TensorRef& in, const TensorRef& out, int batch, int act_dtype, cudaStream_t st);

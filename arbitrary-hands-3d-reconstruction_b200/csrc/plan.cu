@@ -39,6 +39,7 @@ static int make_conv_args(const acr_b200_op& op, int batch, char* arena, const c
   a->pow11_ch0 = (op.shift[0] & ACR_CONV_POW11_CH0) ? 1 : 0;
   a->xpair = (op.shift[0] & ACR_CONV_XPAIR) ? 1 : 0;
   a->s2x = (op.shift[0] & ACR_CONV_S2X) ? 1 : 0;
+  a->deconv = (op.shift[0] & ACR_CONV_DECONV) ? 1 : 0;
   a->n_ext = 0;
   if (op.shift[0] & ACR_CONV_EXTRA) {
     ACR_CHECK_ARG(!op.has_residual && op.n_in >= 2 && op.n_in <= 4, "conv: extra terms need 2..4 inputs and no residual");
@@ -55,10 +56,16 @@ static int make_conv_args(const acr_b200_op& op, int batch, char* arena, const c
     ACR_CHECK_ARG(op.aux[0].dtype == ACR_DT_F32 && op.aux[0].pix_stride >= op.cout_pad, "conv: per-image bias tensor (aux[0]) malformed");
     a->bias = reinterpret_cast<const float*>(arena + op.aux[0].offset);
   }
-  ACR_CHECK_ARG((op.k == 1 || op.k == 3) && (op.stride == 1 || op.stride == 2), "conv: k/stride unsupported");
-  if (a->s2x) ACR_CHECK_ARG(op.stride == 2 && a->out.H * 2 == a->in.H && a->out.W == a->in.W, "conv: x-paired stride-2 spatial mismatch");
-  else ACR_CHECK_ARG(a->out.H * op.stride == a->in.H && a->out.W * op.stride == a->in.W, "conv: spatial mismatch");
-  ACR_CHECK_ARG(op.cout_pad % 16 == 0 && op.cin_pad % 16 == 0 && op.cout_pad <= 1024, "conv: padded channel counts");
+  if (a->deconv) {
+    ACR_CHECK_ARG(op.k == 4 && op.stride == 2 && !op.has_residual && !(op.shift[0] & (ACR_CONV_EXTRA | ACR_CONV_XPAIR | ACR_CONV_S2X)) &&
+                      a->out.H == 2 * a->in.H && a->out.W == 2 * a->in.W,
+                  "conv: the transposed conv is k4 s2 (output 2H x 2W) without residual, extra terms or x-pairing");
+  } else {
+    ACR_CHECK_ARG((op.k == 1 || op.k == 3) && (op.stride == 1 || op.stride == 2), "conv: k/stride unsupported");
+    if (a->s2x) ACR_CHECK_ARG(op.stride == 2 && a->out.H * 2 == a->in.H && a->out.W == a->in.W, "conv: x-paired stride-2 spatial mismatch");
+    else ACR_CHECK_ARG(a->out.H * op.stride == a->in.H && a->out.W * op.stride == a->in.W, "conv: spatial mismatch");
+  }
+  ACR_CHECK_ARG(op.cout_pad % 16 == 0 && op.cin_pad % 16 == 0 && op.cout_pad <= 2048 && op.cin_pad <= 2048, "conv: padded channel counts");
   ACR_CHECK_ARG(a->out.pix_stride >= op.cout_pad, "conv: output buffer narrower than cout_pad");
   return ACR_B200_OK;
 }
@@ -77,8 +84,12 @@ static int run_one_f32(const acr_b200_op& op, int batch, char* arena, const char
       ConvArgs a;
       int rc = make_conv_args(op, batch, arena, weights, external, &a);
       if (rc) return rc;
+      if (a.deconv) { set_error("conv: the fp32 validation plan has no transposed conv"); return ACR_B200_ENOTSUP; }
       return launch_conv_f32(a, st);
     }
+    case ACR_OP_MAXPOOL:
+      set_error("max-pool (ResNet trunk) has no fp32 validation kernel");
+      return ACR_B200_ENOTSUP;
     case ACR_OP_FUSE: {
       FuseArgs f;
       f.out = resolve(op.out, arena, external);
@@ -96,7 +107,7 @@ static int run_one_f32(const acr_b200_op& op, int batch, char* arena, const char
                              reinterpret_cast<float*>(arena + op.out.offset), batch, st);
     default:
       set_error("op kind %d has no fp32 validation kernel", op.kind);
-      return ACR_B200_EINVAL;
+      return op.kind == ACR_OP_STEM_TC && op.k == 7 ? ACR_B200_ENOTSUP : ACR_B200_EINVAL;
   }
 }
 
@@ -113,7 +124,9 @@ static int run_one(const acr_b200_op& op, int batch, char* arena, const char* we
     case ACR_OP_STEM_TC:
       ACR_CHECK_ARG(external != nullptr, "stem_tc: external image pointer is null");
       return launch_stem_tc(resolve(op.in[0], arena, external), resolve(op.out, arena, external), weights + op.w_offset[0],
-                            reinterpret_cast<const float*>(weights + op.w_offset[1]), batch, act_dtype, st);
+                            reinterpret_cast<const float*>(weights + op.w_offset[1]), batch, act_dtype, op.k == 7 ? 7 : 3, st);
+    case ACR_OP_MAXPOOL:
+      return launch_maxpool(resolve(op.in[0], arena, external), resolve(op.out, arena, external), batch, act_dtype, st);
     case ACR_OP_IM2COL_STEM:
       ACR_CHECK_ARG(external != nullptr, "im2col_stem: external image pointer is null");
       return launch_im2col_stem(resolve(op.in[0], arena, external), resolve(op.out, arena, external), batch, act_dtype, st);
@@ -133,6 +146,10 @@ static int run_one(const acr_b200_op& op, int batch, char* arena, const char* we
       ConvArgs a;
       int rc = make_conv_args(op, batch, arena, weights, external, &a);
       if (rc) return rc;
+      if (a.deconv || (a.k == 1 && a.stride == 2) || a.cout_pad > 1024 || a.cin_pad > 1024) {
+        set_error("conv_ref: no CUDA-core form of the transposed conv, the 1x1 stride-2 conv or channels beyond 1024");
+        return ACR_B200_ENOTSUP;
+      }
       return launch_conv_ref(a, act_dtype, st);
     }
     case ACR_OP_FUSE: {

@@ -200,9 +200,11 @@ enum {
   ACR_OP_CONV_REF = 8,    /* debug: same contract as ACR_OP_CONV on CUDA cores (tests only)     */
   ACR_OP_FINALCONV = 9,   /* (retired)                                                          */
   ACR_OP_IM2COL_STEM = 10, /* uint8 NHWC image -> 3x3 s2 im2col of x/255*2-1, 27(+5 zero) 16-bit channels */
-  ACR_OP_STEM_TC = 11      /* STEM on the tensor cores: the im2col operand is built in shared memory, never in HBM   */
-};
-enum { ACR_CONV_BIAS_PER_IMAGE = 1, ACR_CONV_POW11_CH0 = 2, ACR_CONV_XPAIR = 4, ACR_CONV_S2X = 8, ACR_CONV_EXTRA = 16 };
+  ACR_OP_STEM_TC = 11,     /* STEM on the tensor cores: the im2col operand is built in shared memory, never in HBM   */
+  ACR_OP_MAXPOOL = 12      /* nn.MaxPool2d(3, stride 2, padding 1) on 16-bit NHWC (ResNet trunk)                     */
+};  /* kinds stay below 16: acr_b200_plan_profile indexes ms_by_kind[16] */
+enum { ACR_CONV_BIAS_PER_IMAGE = 1, ACR_CONV_POW11_CH0 = 2, ACR_CONV_XPAIR = 4, ACR_CONV_S2X = 8, ACR_CONV_EXTRA = 16,
+       ACR_CONV_DECONV = 32 };
 enum { ACR_DT_BF16 = 0, ACR_DT_F16 = 1, ACR_DT_F32 = 2, ACR_DT_U8 = 3 };
 
 typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image extents)  */
@@ -217,7 +219,13 @@ typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image
  *  STEM      in[0]=image(u8,external) out; w_offset[0]=fp32 [27][64] folded weights, [1]=fp32 bias[64]
  *  STEM_TC   in[0]=image(u8,external) out (64 ch, H/2 x W/2, 16-bit); w_offset[0]=packed [64][32] 16-bit weights (input
  *            channel (ky*3+kx)*3+ci, 27..31 zero, BN folded), [1]=fp32 bias[64]: conv1 + bn1 + ReLU of acr/model.py:832-835
- *            as one wgmma GEMM whose A operand (the 27 normalised taps of every output pixel) is built in shared memory
+ *            as one wgmma GEMM whose A operand (the 27 normalised taps of every output pixel) is built in shared memory.
+ *            k = 7: the ResNet stem instead, conv1 7x7 stride 2 padding 3 (3 -> 64) + bn1 + ReLU; w_offset[0] = packed
+ *            [64][160] (input channel (ky*7+kx)*3+ci, 147..159 zero, BN folded).  Any other k (0 included) = 3x3.
+ *            Both forms pad with zeros (not -1) and carry the bias in spare K channels.  The output tiles per row and
+ *            per image must be powers of two.
+ *  MAXPOOL   in[0] (16-bit NHWC, C and pix_stride multiples of 8) -> out (H/2 x W/2, same dtype): max over the
+ *            valid taps of the 3x3 window at (2y-1.., 2x-1..) (padding never wins, as nn.MaxPool2d(3, 2, 1))
  *  IM2COL_STEM in[0]=image(u8,external) out (32 ch, H/2 x W/2): channel (ky*3+kx)*3+ci = normalised tap,
  *            0 outside the image; the stem conv then runs as a 1x1 CONV on the tensor cores
  *  CONV(_REF) in[0]=x, in[1]=residual (has_residual) out; w_offset[0]=packed 16-bit weights
@@ -233,7 +241,19 @@ typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image
  *            | ACR_CONV_S2X (3x3 STRIDE-2 conv of a dense 32-channel tensor: in[0] is its x-paired view (H, W/2, 64) --
  *            even pixel's channels then the odd neighbour's in one 128-byte row -- `out` is (H/2, W/2); the packed
  *            weights [cout_pad][9][64] carry the 32 input channels of tap (ky,kx) at K offset 32*(kx != 1))
- *  FUSE      in[0..n_in) with shift[i]; out
+ *            | ACR_CONV_DECONV (nn.ConvTranspose2d(kernel 4, stride 2, padding 1, no bias) + BN (+ReLU): k = 4,
+ *            stride = 2, `out` is (2H, 2W), cin_pad a multiple of 64, no residual / extra terms.  Output pixel
+ *            (2m+py, 2n+px) is a 2x2 conv of the input at row offsets {-1, 0} (py = 0: ky = 3, 1) or {0, +1} (py = 1:
+ *            ky = 2, 0), the same along x.  The packed weights are [4 parities py*2+px][cout_pad][4 taps ty*2+tx]
+ *            [cin_pad], tap (ty,tx) of parity (py,px) = w[ci][co][3-py-2ty][3-px-2tx] of the (cin, cout, 4, 4)
+ *            ConvTranspose2d weight, BN folded; w_offset[1] = fp32 bias[cout_pad].  Output rows may be a channel slice
+ *            of a wider buffer (pix_stride >= cout_pad).)
+ *            Contracts of the tensor-core CONV: k in {1, 3} (4 with ACR_CONV_DECONV), stride in {1, 2}; a 1x1
+ *            stride-2 conv (ResNet downsample, padding 0) reads input pixel (2y, 2x); cin_pad and cout_pad are
+ *            multiples of 16 up to 2048 (K per tap up to 2048, N up to 2048 as 16 balanced virtual tiles of 128).
+ *            The fp32 validation plan and CONV_REF take neither ACR_CONV_DECONV, MAXPOOL nor the k = 7 stem:
+ *            they return ACR_B200_ENOTSUP.
+ *  FUSE     in[0..n_in) with shift[i]; out
  *  BILINEAR2X / COORD (fparam unused; COORD writes channels [in[0].C, pix_stride) of `out`)
  *  POOL      in[0]=contact features (256ch), in[1]=segm logits; out = partials (fp32, 1x1xC)
  *  PARTHEAD  in[0]=partials; out=pooled (fp32 256*32); aux[0..1]=bias_img l,r (112); aux[2..3]=

@@ -2,6 +2,8 @@
 """Per-layer-class table of the conv launch set of one bench step, timed with CUDA events (Engine.profile_ops):
     python tools/conv_layers.py [--batch 256] [--warmup 2] [--passes 5]
     python tools/conv_layers.py --dry-run        shapes, FLOP, bytes and floors only (no GPU needed)
+    python tools/conv_layers.py --backbone resnet50   the ResNet-50 trunk's plan (transposed convs are a class of their
+                                                      own, k shown as "4T", FLOP by live taps)
 
 Conv launches are grouped by (cin, cout, k, s, H_in, residual).  Per class: launches, device ms (the median of every
 launch over the profiled passes, summed), TFLOP/s, algorithmic GB/s (input + output (+ residual) (+ extra terms) once),
@@ -62,10 +64,12 @@ def conv_classes(recs, batch):
             continue
         x, y, at = r["ins"][0], r["out"], r["attrs"]
         cin = 109 if "fold_side" in at else (27 if "stem" in at else x.C)   # real input channels of the GEMM
-        key = (cin, y.C, at["k"], at["s"], x.H, bool(at["residual"]))
+        deconv = bool(at.get("deconv"))
+        taps = 4 if deconv else at["k"] ** 2                                  # transposed conv: 2x2 live taps per pixel
+        key = (cin, y.C, f"{at['k']}T" if deconv else at["k"], at["s"], x.H, bool(at["residual"]))
         a = agg.setdefault(key, [[], 0.0, 0.0, 0.0])
         a[0].append(i)
-        a[1] += 2.0 * y.H * y.W * y.C * cin * at["k"] ** 2 * batch / 1e9
+        a[1] += 2.0 * y.H * y.W * y.C * cin * taps * batch / 1e9
         nbytes = batch * (x.H * x.W * x.C * 2 + y.H * y.W * y.C * (4 if y.dtype == "f32" else 2) * (2 if at["residual"] else 1))
         if at.get("extra"):
             nbytes += sum(batch * t.H * t.W * t.C * 2 for t in r["ins"][1:])
@@ -83,11 +87,12 @@ def main():
     ap.add_argument("--sm-mhz", type=float, default=None, help="SM clock of the compute floor (default: sampled; 1600 dry)")
     ap.add_argument("--sms", type=int, default=132)
     ap.add_argument("--dry-run", action="store_true", help="no GPU: shapes, FLOP, bytes and floors without times")
+    ap.add_argument("--backbone", choices=["hrnet", "resnet50"], default="hrnet", help="trunk of the plan (HRNet-W32 default)")
     args = ap.parse_args()
 
     ms_op = None
     if args.dry_run:
-        eng = Engine(None, args.batch, "cpu", dry_run=True)
+        eng = Engine(None, args.batch, "cpu", dry_run=True, backbone=args.backbone)
         mhz = args.sm_mhz or 1600.0
         print(f"dry run (no GPU): batch {args.batch}, floors at {args.sms} SMs x {mhz:.0f} MHz and {args.hbm_gbs:.0f} GB/s")
     else:
@@ -95,8 +100,12 @@ def main():
         from acr_b200.synth import load_bn_calibration, synth_state_dict
         dev = torch.device("cuda", torch.cuda.current_device())
         name, plimit = smi("name,power.limit", dev.index)[:2]
-        sd = synth_state_dict(0, bn_stats=load_bn_calibration(0))
-        eng = Engine(sd, args.batch, dev, torch.bfloat16, 512)
+        if args.backbone == "resnet50":
+            from acr_b200.netspec import build_acr_spec
+            sd = synth_state_dict(0, spec=build_acr_spec(512, backbone="resnet50"))
+        else:
+            sd = synth_state_dict(0, bn_stats=load_bn_calibration(0))
+        eng = Engine(sd, args.batch, dev, torch.bfloat16, 512, backbone=args.backbone)
         frames = torch.randint(0, 256, (args.batch, 512, 512, 3), generator=torch.Generator().manual_seed(1000),
                                dtype=torch.uint8).to(dev)
         for _ in range(args.warmup):
