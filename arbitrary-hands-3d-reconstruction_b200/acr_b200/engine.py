@@ -333,6 +333,47 @@ class Engine:
                 self.arena_bytes = max(self.arena_bytes, g["offset"] + _rup(g["bytes"], ALIGN))
         self.geo = geo
         self.n_ops = len(recs)
+
+        def pairable(r) -> bool:
+            """3x3 stride-1 32->32 convs on dense tensors run as 64->64 convs on the x-paired grid: same
+            bytes in memory, but 128-byte operand rows (SWIZZLE_128B) instead of 64-byte ones."""
+            a = r.get("attrs", {})
+            if self.f32 or r["kind"] not in (L.OP_CONV, L.OP_CONV_REF) or "fold_side" in a or a.get("k") != 3 or a.get("s") != 1:
+                return False
+            ts = r["ins"] + [r["out"]]
+            return all(t.C == 32 and t.base is None and t.dtype == "act" and t.W % 32 == 0 for t in ts)
+
+        def block_pair(i) -> bool:
+            """recs i, i + 1 are one BasicBlock that the fused kernel takes (csrc/conv_block.cuh): conv3x3-BN-ReLU, then
+            conv3x3-BN + the block input, ReLU, both 64 -> 64 or both x-paired 32 -> 32, and nothing else reads the
+            intermediate."""
+            if self.f32 or i + 1 >= len(recs):
+                return False
+            r1, r2 = recs[i], recs[i + 1]
+            if r1["kind"] != L.OP_CONV or r2["kind"] != L.OP_CONV:
+                return False
+            a1, a2 = r1.get("attrs", {}), r2.get("attrs", {})
+            special = ("extra", "merged", "fold_side", "stem", "deconv", "pow11")
+            if any(a.get(k) for a in (a1, a2) for k in special):
+                return False
+            if not all(a.get("k") == 3 and a.get("s") == 1 and a.get("relu") for a in (a1, a2)):
+                return False
+            x, y = r1["ins"][0], r1["out"]
+            if a1.get("residual") or not a2.get("residual") or len(r2["ins"]) != 2 \
+                    or r2["ins"][0] is not y or r2["ins"][1] is not x:
+                return False
+            if y.base is not None or last_use[y.name] != i + 1:
+                return False
+            if pairable(r1) and pairable(r2):
+                return True
+            return x.C == y.C == r2["out"].C == 64 and x.dtype == y.dtype == r2["out"].dtype == "act"
+
+        # BasicBlocks run as one launch each; the records stay one per spec op
+        self.block_starts = [i for i in range(len(recs)) if block_pair(i)]
+        for i in self.block_starts:
+            recs[i]["block"] = True
+            recs[i]["block_mid"] = not reuse_memory or recs[i]["out"].name in keep_roots
+
         if self.dry_run:
             return
 
@@ -357,15 +398,6 @@ class Engine:
             x, y = r["ins"][0], r["out"]
             return (x.C == 32 and x.base is None and x.dtype == "act" and x.W % 32 == 0 and y.H % 16 == 0 and y.W % 16 == 0
                     and os.environ.get("ACR_B200_S2X", "1") != "0")
-
-        def pairable(r) -> bool:
-            """3x3 stride-1 32->32 convs on dense tensors run as 64->64 convs on the x-paired grid: same
-            bytes in memory, but 128-byte operand rows (SWIZZLE_128B) instead of 64-byte ones."""
-            a = r.get("attrs", {})
-            if self.f32 or r["kind"] not in (L.OP_CONV, L.OP_CONV_REF) or "fold_side" in a or a.get("k") != 3 or a.get("s") != 1:
-                return False
-            ts = r["ins"] + [r["out"]]
-            return all(t.C == 32 and t.base is None and t.dtype == "act" and t.W % 32 == 0 for t in ts)
 
         # ---- weights + C op records
         f32 = lambda k: np.ascontiguousarray(sd[k], np.float32)
@@ -445,6 +477,8 @@ class Engine:
                     o.w_offset[0], o.w_offset[1] = self._pack_conv(sd, blob, a["w"], a["bn"], a["bias"], o.cin_pad, o.cout_pad)
                     if a.get("pow11"):
                         o.shift[0] |= 2  # ACR_CONV_POW11_CH0
+                if r.get("block"):
+                    o.shift[0] |= L.CONV_BLOCK | (L.CONV_BLOCK_MID if r["block_mid"] else 0)
             elif r["kind"] == L.OP_STEM_TC:
                 # weights (64,3,k,k) OIHW -> (64, K, 1, 1) with input channel (ky*k+kx)*3+ci, K = 32 (3x3) or 160 (7x7: k = 7
                 # in the op); BN folded by pack_conv
@@ -545,8 +579,9 @@ class Engine:
         return {k: (float(ms[k]), int(cnt[k])) for k in range(16) if cnt[k]}
 
     def profile_ops(self, image: torch.Tensor) -> np.ndarray:
-        """One serialised, event-bracketed pass: device ms of every launch, in the order of ``recs``."""
-        ms = np.zeros(self.num_launches, np.float32)
+        """One serialised, event-bracketed pass: device ms of every record, in the order of ``recs``.  The two convs of a
+        fused BasicBlock are one launch: its time is on the first, the second reads 0 (``launch_of_rec``)."""
+        ms = np.zeros(self.n_ops, np.float32)
         with torch.cuda.device(self.device):
             L.check(self.lib.acr_b200_plan_profile_ops(self.plan, image.data_ptr(), self._stream(), ms.ctypes.data),
                     "plan_profile_ops")
@@ -555,6 +590,12 @@ class Engine:
     @property
     def num_launches(self) -> int:
         return int(self.lib.acr_b200_plan_num_launches(self.plan))
+
+    def launch_of_rec(self) -> np.ndarray:
+        """Index of the launch that computes each record (the two convs of a fused BasicBlock share one)."""
+        out = np.zeros(self.n_ops, np.int32)
+        L.check(self.lib.acr_b200_plan_op_launch(self.plan, out.ctypes.data), "plan_op_launch")
+        return out
 
     # ------------------------------------------------------------------ outputs
     def view(self, name) -> torch.Tensor:

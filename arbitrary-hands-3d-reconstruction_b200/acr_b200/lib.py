@@ -17,6 +17,8 @@ OK = 0
 OP_STEM, OP_CONV, OP_FUSE, OP_BILINEAR2X, OP_COORD, OP_POOL, OP_PARTHEAD, OP_CONV_REF, OP_FINALCONV, OP_IM2COL_STEM, OP_STEM_TC = range(1, 12)
 OP_MAXPOOL = 12
 CONV_DECONV = 32      # ACR_CONV_DECONV flag bit (shift[0]) of a CONV op
+CONV_BLOCK = 64       # ACR_CONV_BLOCK: this conv and the next are one BasicBlock, run as one launch
+CONV_BLOCK_MID = 128  # ACR_CONV_BLOCK_MID: the fused launch also writes the block's intermediate
 DT_BF16, DT_F16, DT_F32, DT_U8 = 0, 1, 2, 3
 
 
@@ -59,7 +61,7 @@ _lib: Optional[C.CDLL] = None
 
 EXPORTS = ["acr_b200_last_error", "acr_b200_version", "acr_b200_mano_model_floats", "acr_b200_mano_pack_model",
            "acr_b200_mano_forward", "acr_b200_mano_forward_gather", "acr_b200_gather_wait", "acr_b200_cam_trans", "acr_b200_preprocess", "acr_b200_one_euro_state_floats", "acr_b200_one_euro_smooth", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse",
-           "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_profile_ops", "acr_b200_plan_num_launches", "acr_b200_plan_destroy",
+           "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_profile_ops", "acr_b200_plan_num_launches", "acr_b200_plan_op_launch", "acr_b200_plan_destroy",
            "acr_b200_run_op", "acr_b200_pack_conv"]
 
 
@@ -94,6 +96,7 @@ def load() -> C.CDLL:
     lib.acr_b200_plan_profile.argtypes = [vp, vp, vp, vp, vp]
     lib.acr_b200_plan_profile_ops.argtypes = [vp, vp, vp, vp]
     lib.acr_b200_plan_num_launches.argtypes = [vp]
+    lib.acr_b200_plan_op_launch.argtypes = [vp, vp]
     lib.acr_b200_plan_destroy.argtypes = [vp]
     lib.acr_b200_plan_destroy.restype = None
     lib.acr_b200_run_op.argtypes = [C.POINTER(Op), i32, vp, vp, vp, i32, vp]

@@ -1,5 +1,6 @@
-// Host side of the implicit-GEMM conv (conv_tc.cuh): tensor maps, N split, shared-memory plan, launch dispatch.
-#include "conv_tc.cuh"
+// Host side of the implicit-GEMM conv (conv_tc.cuh): tensor maps, N split, shared-memory plan, launch dispatch; and of
+// the fused BasicBlock (conv_block.cuh).
+#include "conv_block.cuh"
 
 namespace acr {
 
@@ -210,5 +211,52 @@ int conv_tc_launch(const ConvTcPlan* pl, cudaStream_t st) {
 }
 
 void conv_tc_free(ConvTcPlan* p) { delete p; }
+
+int conv_block_prepare(const ConvArgs& a1, const ConvArgs& a2, int act_dtype, int store_mid, ConvBlockPlan** out) {
+  auto is_3x3_64 = [&](const ConvArgs& a) {
+    return a.k == 3 && a.stride == 1 && a.cin_pad == 64 && a.cout_pad == 64 && a.relu && !a.bias_per_image && !a.pow11_ch0 &&
+           a.n_ext == 0 && !a.s2x && !a.deconv && a.in.dtype == act_dtype && a.out.dtype == act_dtype;
+  };
+  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16, "conv_block: 16-bit activations only");
+  ACR_CHECK_ARG(is_3x3_64(a1) && is_3x3_64(a2) && !a1.has_res && a2.has_res && a1.xpair == a2.xpair,
+                "conv_block: a BasicBlock of two 3x3 stride-1 64->64 convs (or their x-paired form), ReLU, residual on conv2");
+  ACR_CHECK_ARG(a2.in.ptr == a1.out.ptr && a2.res.ptr == a1.in.ptr && a2.res.pix_stride == a1.in.pix_stride,
+                "conv_block: conv2 must read conv1's output, with conv1's input as the residual");
+  const int H = a1.in.H, W = a1.in.W;
+  ACR_CHECK_ARG(a1.out.H == H && a1.out.W == W && a2.out.H == H && a2.out.W == W && H % TILE_Y == 0 && W % TILE_X == 0,
+                "conv_block: %dx%d is not a multiple of the 16x16 super-tile", H, W);
+  ACR_CHECK_ARG(a1.in.pix_stride % 8 == 0 && a1.in.pix_stride >= 64 && a2.out.pix_stride % 2 == 0 && a1.out.pix_stride % 2 == 0,
+                "conv_block: row alignment");
+  ConvBlockPlan* pl = new ConvBlockPlan();
+  ConvBlockParams& p = pl->p;
+  pl->act_dtype = act_dtype; pl->xpair = a1.xpair;
+  const cuuint64_t esz = 2;
+  int rc;
+  {
+    cuuint64_t dims[4] = {64, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)a1.batch};
+    cuuint64_t str[3] = {(cuuint64_t)a1.in.pix_stride * esz, (cuuint64_t)W * a1.in.pix_stride * esz,
+                         (cuuint64_t)H * W * a1.in.pix_stride * esz};
+    cuuint32_t box[4] = {64, BLK_PITCH, BLK_ROWS, 1};
+    rc = encode(&p.tmA, act_dtype, 4, a1.in.ptr, dims, str, box, 64);
+  }
+  for (int c = 0; c < 2 && !rc; ++c) {
+    cuuint64_t dims[2] = {9 * 64, 64};
+    cuuint64_t str[1] = {9 * 64 * esz};
+    cuuint32_t box[2] = {64, 64};
+    rc = encode(c ? &p.tmB2 : &p.tmB1, act_dtype, 2, c ? a2.w : a1.w, dims, str, box, 64);
+  }
+  if (rc) { delete pl; return rc; }
+  p.bias1 = a1.bias; p.bias2 = a2.bias;
+  p.res = a2.res.ptr; p.out = a2.out.ptr; p.mid = store_mid ? a1.out.ptr : nullptr;
+  p.res_stride = a2.res.pix_stride; p.out_stride = a2.out.pix_stride; p.mid_stride = a1.out.pix_stride;
+  p.H = H; p.W = W;
+  p.tiles_x = W / TILE_X; p.tiles_per_img = p.tiles_x * (H / TILE_Y);
+  p.total_tiles = p.tiles_per_img * a1.batch;
+  pl->grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
+  *out = pl;
+  return ACR_B200_OK;
+}
+
+void conv_block_free(ConvBlockPlan* p) { delete p; }
 
 }  // namespace acr

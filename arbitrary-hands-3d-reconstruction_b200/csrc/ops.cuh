@@ -77,5 +77,10 @@ struct ConvTcPlan;   // holds the TMA tensor maps of one conv op
 int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out);
 int conv_tc_launch(const ConvTcPlan* p, cudaStream_t st);
 void conv_tc_free(ConvTcPlan* p);
+// one HRNet BasicBlock (two 3x3 64->64 convs, or their x-paired form, + residual) as one launch (conv_block.cuh)
+struct ConvBlockPlan;
+int conv_block_prepare(const ConvArgs& a1, const ConvArgs& a2, int act_dtype, int store_mid, ConvBlockPlan** out);
+int conv_block_launch(const ConvBlockPlan* p, cudaStream_t st);
+void conv_block_free(ConvBlockPlan* p);
 
 }  // namespace acr

@@ -197,6 +197,9 @@ constexpr int MAX_STREAMS = 8;
 struct acr_b200_plan {
   std::vector<acr_b200_op> ops;
   std::vector<ConvTcPlan*> tc;
+  std::vector<ConvBlockPlan*> blk;     // op i (ACR_CONV_BLOCK) launches the fused BasicBlock of ops i and i + 1
+  std::vector<char> fused;             // op i is the second conv of a fused block: no launch of its own
+  int n_launches = 0;
   int batch = 0, act_dtype = 0, n_streams = 1;
   char* arena = nullptr;
   size_t arena_bytes = 0;
@@ -205,6 +208,20 @@ struct acr_b200_plan {
   std::vector<cudaEvent_t> ev_op;      // one event per op (recorded when some later op waits on its stream)
   cudaEvent_t ev_begin = nullptr;
 };
+
+// Fused BasicBlocks (ACR_CONV_BLOCK) are on by default; ACR_B200_FUSE_BLOCKS=0 (read at plan creation) launches the two
+// convs of every block separately again (A/B timing).
+static bool fuse_blocks_enabled() {
+  const char* e = getenv("ACR_B200_FUSE_BLOCKS");
+  return !(e && atoi(e) == 0);
+}
+
+// the launch of op i: nothing for the second conv of a fused block, the fused kernel for its first
+static int launch_op(acr_b200_plan* p, int i, const void* image, cudaStream_t st) {
+  if (p->fused[i]) return ACR_B200_OK;
+  if (p->blk[i]) return conv_block_launch(p->blk[i], st);
+  return run_one(p->ops[i], p->batch, p->arena, p->weights, static_cast<const char*>(image), p->act_dtype, p->tc[i], st);
+}
 
 extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch, void* arena,
                                     size_t arena_bytes, const void* weights, size_t weight_bytes,
@@ -216,6 +233,8 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
   ACR_CHECK_ARG(p != nullptr, "plan_create: out of host memory");
   p->ops.assign(ops, ops + n_ops);
   p->tc.assign(n_ops, nullptr);
+  p->blk.assign(n_ops, nullptr);
+  p->fused.assign(n_ops, 0);
   p->batch = batch; p->act_dtype = act_dtype;
   p->arena = static_cast<char*>(arena); p->arena_bytes = arena_bytes;
   p->weights = static_cast<const char*>(weights);
@@ -230,6 +249,23 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
       const size_t need = op.out.offset + (size_t)batch * op.out.H * op.out.W * op.out.pix_stride * esz;
       if (need > arena_bytes) { set_error("op %d: output exceeds the arena (%zu > %zu)", i, need, arena_bytes); rc = ACR_B200_EINVAL; break; }
     }
+    if (p->fused[i]) continue;
+    if (op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32 && (op.shift[0] & ACR_CONV_BLOCK) && fuse_blocks_enabled()) {
+      // one launch for the BasicBlock of ops i and i + 1 (the engine marks only such pairs); op i + 1's waits must be
+      // ones op i already has, so nothing that op i + 1 waited for can be missed
+      if (!(i + 1 < n_ops && p->ops[i + 1].kind == ACR_OP_CONV && p->ops[i + 1].stream_id == op.stream_id &&
+            (p->ops[i + 1].wait_mask & ~op.wait_mask & ~(1 << op.stream_id)) == 0)) {
+        set_error("op %d: ACR_CONV_BLOCK needs the block's second conv next, on the same stream", i);
+        rc = ACR_B200_EINVAL;
+        break;
+      }
+      ConvArgs a1, a2;
+      rc = make_conv_args(op, batch, p->arena, p->weights, nullptr, &a1);
+      if (rc == ACR_B200_OK) rc = make_conv_args(p->ops[i + 1], batch, p->arena, p->weights, nullptr, &a2);
+      if (rc == ACR_B200_OK) rc = conv_block_prepare(a1, a2, act_dtype, (op.shift[0] & ACR_CONV_BLOCK_MID) ? 1 : 0, &p->blk[i]);
+      p->fused[i + 1] = 1;
+      continue;
+    }
     if (op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32) {
       ConvArgs a;
       rc = make_conv_args(op, batch, p->arena, p->weights, nullptr, &a);
@@ -237,6 +273,7 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
     }
   }
   if (rc == ACR_B200_OK) {
+    for (int i = 0; i < n_ops; ++i) p->n_launches += p->fused[i] ? 0 : 1;
     for (int s = 1; s < p->n_streams && rc == ACR_B200_OK; ++s)
       if (cudaStreamCreateWithFlags(&p->streams[s], cudaStreamNonBlocking) != cudaSuccess) { set_error("plan_create: cudaStreamCreate failed"); rc = ACR_B200_ECUDA; }
     p->ev_op.assign(n_ops, nullptr);
@@ -259,8 +296,7 @@ extern "C" int acr_b200_plan_run(acr_b200_plan* p, const void* image, void* stre
     // ACR_B200_DEBUG_SYNC=1: synchronise after every launch and name the op that failed (debugging only)
     static const bool debug_sync = [] { const char* e = getenv("ACR_B200_DEBUG_SYNC"); return e && atoi(e) != 0; }();
     for (int i = 0; i < n; ++i) {
-      int rc = run_one(p->ops[i], p->batch, p->arena, p->weights,
-                       static_cast<const char*>(image), p->act_dtype, p->tc[i], main_st);
+      int rc = launch_op(p, i, image, main_st);
       if (rc) return rc;
       if (debug_sync) {
         cudaError_t e = cudaStreamSynchronize(main_st);
@@ -290,7 +326,7 @@ extern "C" int acr_b200_plan_run(acr_b200_plan* p, const void* image, void* stre
       if ((op.wait_mask >> s) & 1) {
         if (s != op.stream_id && last_on[s] >= 0) ACR_CHECK_CUDA(cudaStreamWaitEvent(st, p->ev_op[last_on[s]], 0));
       }
-    int rc = run_one(op, p->batch, p->arena, p->weights, static_cast<const char*>(image), p->act_dtype, p->tc[i], st);
+    int rc = launch_op(p, i, image, st);
     if (rc) return rc;
     ACR_CHECK_CUDA(cudaEventRecord(p->ev_op[i], st));
     last_on[op.stream_id] = i;
@@ -300,7 +336,8 @@ extern "C" int acr_b200_plan_run(acr_b200_plan* p, const void* image, void* stre
   return ACR_B200_OK;
 }
 
-// one serialised pass with an event after every op: device milliseconds of op i into ms_by_op[i]
+// one serialised pass with an event after every op: device milliseconds of op i into ms_by_op[i] (a fused block's time
+// is on its first conv, its second conv reads 0)
 static int profile_ops(acr_b200_plan* p, const void* image, cudaStream_t st, float* ms_by_op) {
   const int n = (int)p->ops.size();
   std::vector<cudaEvent_t> ev(n + 1);
@@ -308,7 +345,7 @@ static int profile_ops(acr_b200_plan* p, const void* image, cudaStream_t st, flo
   ACR_CHECK_CUDA(cudaEventRecord(ev[0], st));
   int rc = ACR_B200_OK;
   for (int i = 0; i < n && rc == ACR_B200_OK; ++i) {
-    rc = run_one(p->ops[i], p->batch, p->arena, p->weights, static_cast<const char*>(image), p->act_dtype, p->tc[i], st);
+    rc = launch_op(p, i, image, st);
     if (rc == ACR_B200_OK && cudaEventRecord(ev[i + 1], st) != cudaSuccess) rc = ACR_B200_ECUDA;
   }
   if (rc == ACR_B200_OK && cudaStreamSynchronize(st) != cudaSuccess) { set_error("plan_profile: sync failed: %s", cudaGetErrorString(cudaGetLastError())); rc = ACR_B200_ECUDA; }
@@ -329,6 +366,7 @@ extern "C" int acr_b200_plan_profile(acr_b200_plan* p, const void* image, void* 
   if (rc == ACR_B200_OK) {
     for (int k = 0; k < 16; ++k) { ms_by_kind[k] = 0.f; n_by_kind[k] = 0; }
     for (size_t i = 0; i < ms.size(); ++i) {
+      if (p->fused[i]) continue;
       const int k = p->ops[i].kind & 15;
       ms_by_kind[k] += ms[i]; n_by_kind[k] += 1;
     }
@@ -341,11 +379,22 @@ extern "C" int acr_b200_plan_profile_ops(acr_b200_plan* p, const void* image, vo
   return profile_ops(p, image, static_cast<cudaStream_t>(stream), ms_by_op);
 }
 
-extern "C" int acr_b200_plan_num_launches(const acr_b200_plan* p) { return p ? (int)p->ops.size() : 0; }
+extern "C" int acr_b200_plan_num_launches(const acr_b200_plan* p) { return p ? p->n_launches : 0; }
+
+extern "C" int acr_b200_plan_op_launch(const acr_b200_plan* p, int32_t* launch_of_op) {
+  ACR_CHECK_ARG(p && launch_of_op, "plan_op_launch: bad arguments");
+  int l = -1;
+  for (size_t i = 0; i < p->ops.size(); ++i) {
+    if (!p->fused[i]) ++l;
+    launch_of_op[i] = l;
+  }
+  return ACR_B200_OK;
+}
 
 extern "C" void acr_b200_plan_destroy(acr_b200_plan* p) {
   if (!p) return;
   for (ConvTcPlan* t : p->tc) conv_tc_free(t);
+  for (ConvBlockPlan* b : p->blk) conv_block_free(b);
   for (int s = 1; s < MAX_STREAMS; ++s)
     if (p->streams[s]) cudaStreamDestroy(p->streams[s]);
   for (cudaEvent_t e : p->ev_op)

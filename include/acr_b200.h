@@ -204,7 +204,7 @@ enum {
   ACR_OP_MAXPOOL = 12      /* nn.MaxPool2d(3, stride 2, padding 1) on 16-bit NHWC (ResNet trunk)                     */
 };  /* kinds stay below 16: acr_b200_plan_profile indexes ms_by_kind[16] */
 enum { ACR_CONV_BIAS_PER_IMAGE = 1, ACR_CONV_POW11_CH0 = 2, ACR_CONV_XPAIR = 4, ACR_CONV_S2X = 8, ACR_CONV_EXTRA = 16,
-       ACR_CONV_DECONV = 32 };
+       ACR_CONV_DECONV = 32, ACR_CONV_BLOCK = 64, ACR_CONV_BLOCK_MID = 128 };
 enum { ACR_DT_BF16 = 0, ACR_DT_F16 = 1, ACR_DT_F32 = 2, ACR_DT_U8 = 3 };
 
 typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image extents)  */
@@ -248,7 +248,13 @@ typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image
  *            [cin_pad], tap (ty,tx) of parity (py,px) = w[ci][co][3-py-2ty][3-px-2tx] of the (cin, cout, 4, 4)
  *            ConvTranspose2d weight, BN folded; w_offset[1] = fp32 bias[cout_pad].  Output rows may be a channel slice
  *            of a wider buffer (pix_stride >= cout_pad).)
- *            Contracts of the tensor-core CONV: k in {1, 3} (4 with ACR_CONV_DECONV), stride in {1, 2}; a 1x1
+ *            | ACR_CONV_BLOCK (this conv and the NEXT op are one HRNet BasicBlock: both 3x3 stride-1 64->64 with ReLU, or
+            both x-paired; the next op reads this op's output, has this op's input as its residual and is the only reader
+            of this op's output.  The plan runs the pair as ONE launch whose intermediate stays in shared memory
+            (csrc/conv_block.cuh); bit-identical to two launches.  ACR_B200_FUSE_BLOCKS=0 in the environment at plan
+            creation ignores the flag)  | ACR_CONV_BLOCK_MID (with ACR_CONV_BLOCK: the fused launch still writes this
+            op's output, for readers outside the plan)
+            Contracts of the tensor-core CONV: k in {1, 3} (4 with ACR_CONV_DECONV), stride in {1, 2}; a 1x1
  *            stride-2 conv (ResNet downsample, padding 0) reads input pixel (2y, 2x); cin_pad and cout_pad are
  *            multiples of 16 up to 2048 (K per tap up to 2048, N up to 2048 as 16 balanced virtual tiles of 128).
  *            The fp32 validation plan and CONV_REF take neither ACR_CONV_DECONV, MAXPOOL nor the k = 7 stem:
@@ -293,10 +299,15 @@ int acr_b200_plan_run(acr_b200_plan* plan, const void* image, void* stream);
 int acr_b200_plan_profile(acr_b200_plan* plan, const void* image, void* stream, float* ms_by_kind,
                           int32_t* n_by_kind);
 /* The same serialised, event-bracketed pass, but writes the device milliseconds of op i into ms_by_op[i]
- * (host array of plan_num_launches floats, in plan order).  Synchronises `stream`.  Per-layer tables. */
+ * (host array of n_ops floats, in plan order; a fused BasicBlock's time is on its first conv, the second reads 0).
+ * Synchronises `stream`.  Per-layer tables.                                                 */
 int acr_b200_plan_profile_ops(acr_b200_plan* plan, const void* image, void* stream, float* ms_by_op);
-/* Number of kernel launches one plan_run issues (for bench.py's gpu_launches).            */
+/* Number of kernel launches one plan_run issues (for bench.py's gpu_launches): the plan's ops less the
+ * second convs of fused BasicBlocks (ACR_CONV_BLOCK).                                       */
 int acr_b200_plan_num_launches(const acr_b200_plan* plan);
+/* launch_of_op[i] (host array of n_ops int32) = index of the launch that computes op i: the two convs of a fused
+ * BasicBlock share one launch.                                                              */
+int acr_b200_plan_op_launch(const acr_b200_plan* plan, int32_t* launch_of_op);
 void acr_b200_plan_destroy(acr_b200_plan* plan);
 
 /* Single-op entry used by the parity tests (same code path as inside a plan).             */

@@ -56,20 +56,35 @@ class ClockSampler(threading.Thread):
         return float(np.median(self.mhz)) if self.mhz else None
 
 
-def conv_classes(recs, batch):
-    """[(key, [rec indices], GFLOP, algorithmic MB, weights KB)] of the conv launches, in plan order of first use."""
+def conv_classes(recs, batch, blocks=()):
+    """[(key, [rec indices], GFLOP, algorithmic MB, weights KB, issued GFLOP)] of the conv launches, in plan order of first
+    use.  `blocks`: first records of the BasicBlocks that run as one fused launch (csrc/conv_block.cuh), a class of their
+    own (k "3+3"): FLOP of both convs, bytes in + out, and the issued FLOP of the fused kernel (conv1 runs 8 M blocks of 64
+    flat rows per 16x16 tile, 2x its pixels; the x-paired form issues its side taps at full width, 4/3)."""
     agg = collections.OrderedDict()
+    blocks = set(blocks)
     for i, r in enumerate(recs):
-        if r["kind"] != L.OP_CONV:
+        if r["kind"] != L.OP_CONV or i - 1 in blocks:
             continue
         x, y, at = r["ins"][0], r["out"], r["attrs"]
+        if i in blocks:
+            key = (x.C, y.C, "3+3", 1, x.H, True)
+            a = agg.setdefault(key, [[], 0.0, 0.0, 0.0, 0.0])
+            a[0] += [i, i + 1]
+            gflop = 2 * 2.0 * y.H * y.W * y.C * x.C * 9 * batch / 1e9
+            a[1] += gflop
+            a[2] += batch * (x.H * x.W * x.C + y.H * y.W * y.C) * 2 / 1e6
+            a[3] = 2 * y.C * x.C * 9 * 2 / 1024
+            a[4] += gflop * 1.5 * (4 / 3 if x.C == 32 else 1)
+            continue
         cin = 109 if "fold_side" in at else (27 if "stem" in at else x.C)   # real input channels of the GEMM
         deconv = bool(at.get("deconv"))
         taps = 4 if deconv else at["k"] ** 2                                  # transposed conv: 2x2 live taps per pixel
         key = (cin, y.C, f"{at['k']}T" if deconv else at["k"], at["s"], x.H, bool(at["residual"]))
-        a = agg.setdefault(key, [[], 0.0, 0.0, 0.0])
+        a = agg.setdefault(key, [[], 0.0, 0.0, 0.0, 0.0])
         a[0].append(i)
         a[1] += 2.0 * y.H * y.W * y.C * cin * taps * batch / 1e9
+        a[4] = a[1]
         nbytes = batch * (x.H * x.W * x.C * 2 + y.H * y.W * y.C * (4 if y.dtype == "f32" else 2) * (2 if at["residual"] else 1))
         if at.get("extra"):
             nbytes += sum(batch * t.H * t.W * t.C * 2 for t in r["ins"][1:])
@@ -93,6 +108,7 @@ def main():
     ms_op = None
     if args.dry_run:
         eng = Engine(None, args.batch, "cpu", dry_run=True, backbone=args.backbone)
+        blocks = eng.block_starts if os.environ.get("ACR_B200_FUSE_BLOCKS", "1") != "0" else []
         mhz = args.sm_mhz or 1600.0
         print(f"dry run (no GPU): batch {args.batch}, floors at {args.sms} SMs x {mhz:.0f} MHz and {args.hbm_gbs:.0f} GB/s")
     else:
@@ -115,6 +131,8 @@ def main():
         runs = np.stack([eng.profile_ops(frames) for _ in range(args.passes)])
         sampled = sampler.stop()
         ms_op = np.median(runs, axis=0)
+        launch = eng.launch_of_rec()
+        blocks = [i for i in eng.block_starts if launch[i] == launch[i + 1]]
         mhz = args.sm_mhz or sampled or 1600.0
         print(f"{name}, power limit {plimit} W, SM clock {sampled if sampled else 'n/a'} MHz (median during the passes); "
               f"batch {args.batch}, median of {args.passes} passes after {args.warmup} warm-up; "
@@ -122,10 +140,10 @@ def main():
 
     peak_tflops = args.sms * FLOP_PER_CLK_SM * mhz * 1e6 / 1e12
     rows = []
-    for key, idx, gflop, mb, wkb in conv_classes(eng.recs, args.batch):
-        t_c, t_m = gflop / peak_tflops, mb / args.hbm_gbs       # ms
+    for key, idx, gflop, mb, wkb, issued in conv_classes(eng.recs, args.batch, blocks):
+        t_c, t_m = issued / peak_tflops, mb / args.hbm_gbs       # ms (compute floor: the FLOP the kernel issues)
         ms = float(ms_op[idx].sum()) if ms_op is not None else None
-        rows.append((key, len(idx), wkb, gflop, mb, t_c, t_m, ms))
+        rows.append((key, len(idx) // (2 if key[2] == "3+3" else 1), wkb, gflop, mb, t_c, t_m, ms))   # launches
     rows.sort(key=lambda r: -(r[7] if r[7] is not None else max(r[5], r[6])))
     head = "| cin | cout | k | s | H_in | res | n | weights KB | GFLOP | MB | compute floor ms | HBM floor ms | bound |"
     if ms_op is not None:
@@ -139,7 +157,7 @@ def main():
         print(line)
     tc, tm = sum(r[5] for r in rows), sum(r[6] for r in rows)
     tf = sum(max(r[5], r[6]) for r in rows)
-    tail = (f"\n{sum(r[1] for r in rows)} conv launches, {sum(r[3] for r in rows):.0f} GFLOP, {sum(r[4] for r in rows) / 1e3:.1f} GB; "
+    tail = (f"\n{sum(r[1] for r in rows)} conv launches ({len(blocks)} fused blocks), {sum(r[3] for r in rows):.0f} GFLOP, {sum(r[4] for r in rows) / 1e3:.1f} GB; "
             f"floors: compute {tc:.1f} ms, HBM {tm:.1f} ms, sum of per-class max {tf:.1f} ms")
     if ms_op is not None:
         t = sum(r[7] for r in rows)
