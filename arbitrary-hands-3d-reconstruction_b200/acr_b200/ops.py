@@ -71,6 +71,32 @@ def mano_forward(model_l: Optional[torch.Tensor], model_r: Optional[torch.Tensor
     return out
 
 
+def mano_backward(model: torch.Tensor, side: int, poses: torch.Tensor, betas: torch.Tensor,
+                  center_idx: Optional[int], dverts: Optional[torch.Tensor], djoints: Optional[torch.Tensor],
+                  dcenter: Optional[torch.Tensor], want_poses: bool = True, want_betas: bool = True):
+    """Gradient of one side's ``mano_forward`` (verts, joints, center) -> (dposes (n,48), dbetas (n,10)); a
+    cotangent of None is zero, an output not wanted comes back as None."""
+    dev = L.require_cuda(model, poses, betas, dverts, djoints, dcenter)
+    n = poses.shape[0]
+    poses = poses.contiguous().float()
+    betas = betas.contiguous().float()
+    dverts, djoints, dcenter = [None if t is None else t.contiguous().float() for t in (dverts, djoints, dcenter)]
+    dposes = torch.empty(n, 48, device=dev) if want_poses else None
+    dbetas = torch.empty(n, 10, device=dev) if want_betas else None
+    if n == 0 or not (want_poses or want_betas):
+        return dposes, dbetas
+    lib = L.load()
+    ws = None
+    if dverts is not None or djoints is not None:
+        ws = torch.empty(int(lib.acr_b200_mano_backward_workspace_floats(n)), device=dev)
+    with L.on(dev):
+        rc = lib.acr_b200_mano_backward(L.ptr(model), int(side), L.ptr(poses), L.ptr(betas), n,
+                                        -1 if center_idx is None else int(center_idx), L.ptr(dverts), L.ptr(djoints),
+                                        L.ptr(dcenter), L.ptr(ws), L.ptr(dposes), L.ptr(dbetas), L.current_stream(dev))
+    L.check(rc, "mano_backward")
+    return dposes, dbetas
+
+
 def cam_trans(j3d: torch.Tensor, pj2d: torch.Tensor, focal_length: float = 1265.0, img_size: float = 512.0,
               n_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(n,21,3), (n,21,2) -> (n,3) camera translation (closed-form least squares on the device)."""

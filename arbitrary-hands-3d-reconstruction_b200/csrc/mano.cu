@@ -135,6 +135,142 @@ __device__ __forceinline__ void write_joint(const ManoParams& p, int hand, int o
   }
 }
 
+// Phase 1, shared by the forward and both backward kernels: thread (h, j) of a 128-thread CTA rebuilds joint j of
+// hand h of the group -- its Rodrigues rotation, rest joint and pose-map rows -- then threads j<5 walk the five
+// fingers (three levels each), and every thread forms its skinning transform A_j.  `m` is the packed model of the
+// hand; a row beyond n (!valid, m unused) gets the identity rotation, a zero joint and zero blend coefficients.
+// Ends synchronised.  kPiTrig as in rodrigues(): the backward kernels use it, so they never touch local memory.
+template <bool kPiTrig = false>
+__device__ __forceinline__ void rebuild_transforms(bool valid, const float* __restrict__ m, const float* __restrict__ poses,
+                                                   const float* __restrict__ betas, int hand, int h, int j, int center_src,
+                                                   float (*s_pm)[HG], float (*s_A)[16][12], float (*s_R)[16][9],
+                                                   float (*s_J)[16][3], float (*s_G)[16][12], float (*s_ctr)[3]) {
+  float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  float J[3] = {0, 0, 0};
+  if (valid) {
+    const float* ps = poses + (size_t)hand * 48 + j * 3;
+    float ax = ps[0] + m[OFF_HM + j * 3 + 0];
+    float ay = ps[1] + m[OFF_HM + j * 3 + 1];
+    float az = ps[2] + m[OFF_HM + j * 3 + 2];
+    rodrigues<kPiTrig>(ax, ay, az, R);
+    const float* b = betas + (size_t)hand * 10;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float a = m[OFF_JT + j * 3 + c];
+      const float* js = m + OFF_JS + (j * 3 + c) * 10;
+#pragma unroll
+      for (int k = 0; k < 10; ++k) a = fmaf(js[k], b[k], a);
+      J[c] = a;
+    }
+    if (j < 10) s_pm[135 + j][h] = b[j];
+  } else if (j < 10) {
+    s_pm[135 + j][h] = 0.f;
+  }
+#pragma unroll
+  for (int e = 0; e < 9; ++e) s_R[h][j][e] = R[e];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) s_J[h][j][c] = J[c];
+  if (j >= 1) {
+#pragma unroll
+    for (int e = 0; e < 9; ++e) s_pm[(j - 1) * 9 + e][h] = valid ? R[e] - ((e & 3) == 0 ? 1.f : 0.f) : 0.f;
+  }
+  __syncthreads();
+  // kinematic chain: thread j<5 walks finger j (joints 3j+1..3j+3); thread j==5 stores the root
+  if (j <= 5) {
+    float G[12];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      G[r * 4 + 0] = s_R[h][0][r * 3 + 0]; G[r * 4 + 1] = s_R[h][0][r * 3 + 1];
+      G[r * 4 + 2] = s_R[h][0][r * 3 + 2]; G[r * 4 + 3] = s_J[h][0][r];
+    }
+    if (j == 5) {
+#pragma unroll
+      for (int e = 0; e < 12; ++e) s_G[h][0][e] = G[e];
+    } else {
+      int parent = 0;
+#pragma unroll
+      for (int lev = 0; lev < 3; ++lev) {
+        const int idx = 3 * j + 1 + lev;
+        const float* Rl = s_R[h][idx];
+        float rel[3] = {s_J[h][idx][0] - s_J[h][parent][0], s_J[h][idx][1] - s_J[h][parent][1],
+                        s_J[h][idx][2] - s_J[h][parent][2]};
+        float N[12];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+          for (int c = 0; c < 3; ++c)
+            N[r * 4 + c] = G[r * 4 + 0] * Rl[0 * 3 + c] + G[r * 4 + 1] * Rl[1 * 3 + c] + G[r * 4 + 2] * Rl[2 * 3 + c];
+          N[r * 4 + 3] = G[r * 4 + 0] * rel[0] + G[r * 4 + 1] * rel[1] + G[r * 4 + 2] * rel[2] + G[r * 4 + 3];
+        }
+#pragma unroll
+        for (int e = 0; e < 12; ++e) { G[e] = N[e]; s_G[h][idx][e] = N[e]; }
+        parent = idx;
+      }
+    }
+  }
+  __syncthreads();
+  // A_j = [R_g | t_g - R_g . J_j]   (manolayer.py:226-228)
+  {
+    const float* G = s_G[h][j];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      s_A[h][j][r * 4 + 0] = G[r * 4 + 0]; s_A[h][j][r * 4 + 1] = G[r * 4 + 1]; s_A[h][j][r * 4 + 2] = G[r * 4 + 2];
+      s_A[h][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[0] + G[r * 4 + 1] * J[1] + G[r * 4 + 2] * J[2]);
+    }
+  }
+  if (j < 3) s_ctr[h][j] = (center_src >= 0) ? s_G[h][center_src][j * 4 + 3] : 0.f;
+  __syncthreads();
+}
+
+// v_posed of vertex column vc for the HG hands of the group: template + 145 blend rows (streamed from L2, coalesced
+// [k][c][v] layout) times the per-hand coefficients broadcast from shared memory.
+__device__ __forceinline__ void blend_vertex(const float* __restrict__ m, int vc, const float (*s_pm)[HG], float (&acc)[HG][3]) {
+  const float* __restrict__ dirs = m + OFF_DIRS;
+  unsigned long long acc2[HG / 2][3];   // (hand 2i, hand 2i+1) packed: one ffma2 (two fp32 FMAs) serves two hands
+  {
+    const float v0 = m[OFF_VT + 0 * NVP + vc], v1 = m[OFF_VT + 1 * NVP + vc], v2 = m[OFF_VT + 2 * NVP + vc];
+#pragma unroll
+    for (int h = 0; h < HG / 2; ++h) { acc2[h][0] = pk2(v0, v0); acc2[h][1] = pk2(v1, v1); acc2[h][2] = pk2(v2, v2); }
+  }
+  // shape rows first (v_shaped), then pose rows, like the reference's evaluation order
+#pragma unroll 5
+  for (int kk = 0; kk < NK; ++kk) {
+    const int k = (kk < 10) ? 135 + kk : kk - 10;
+    const float d0 = __ldg(dirs + ((size_t)k * 3 + 0) * NVP + vc);
+    const float d1 = __ldg(dirs + ((size_t)k * 3 + 1) * NVP + vc);
+    const float d2 = __ldg(dirs + ((size_t)k * 3 + 2) * NVP + vc);
+    const float4 pa = *reinterpret_cast<const float4*>(&s_pm[k][0]);
+    const float4 pb = *reinterpret_cast<const float4*>(&s_pm[k][4]);
+    const unsigned long long D0 = pk2(d0, d0), D1 = pk2(d1, d1), D2 = pk2(d2, d2);
+    const unsigned long long P[4] = {pk2(pa.x, pa.y), pk2(pa.z, pa.w), pk2(pb.x, pb.y), pk2(pb.z, pb.w)};
+#pragma unroll
+    for (int h = 0; h < HG / 2; ++h) {
+      ffma2(acc2[h][0], D0, P[h]);
+      ffma2(acc2[h][1], D1, P[h]);
+      ffma2(acc2[h][2], D2, P[h]);
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < HG / 2; ++h)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) unpk2(acc2[h][c], acc[2 * h][c], acc[2 * h + 1][c]);
+}
+
+// skinning transform of one vertex: T = sum_j w_j A_j (3x4, row-major)
+__device__ __forceinline__ void skin_transform(const float (&w)[16], const float (*A)[12], float (&T)[12]) {
+#pragma unroll
+  for (int e = 0; e < 12; ++e) T[e] = 0.f;
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float4 a0 = *reinterpret_cast<const float4*>(&A[j][0]);
+    const float4 a1 = *reinterpret_cast<const float4*>(&A[j][4]);
+    const float4 a2 = *reinterpret_cast<const float4*>(&A[j][8]);
+    T[0] = fmaf(w[j], a0.x, T[0]); T[1] = fmaf(w[j], a0.y, T[1]); T[2] = fmaf(w[j], a0.z, T[2]); T[3] = fmaf(w[j], a0.w, T[3]);
+    T[4] = fmaf(w[j], a1.x, T[4]); T[5] = fmaf(w[j], a1.y, T[5]); T[6] = fmaf(w[j], a1.z, T[6]); T[7] = fmaf(w[j], a1.w, T[7]);
+    T[8] = fmaf(w[j], a2.x, T[8]); T[9] = fmaf(w[j], a2.y, T[9]); T[10] = fmaf(w[j], a2.z, T[10]); T[11] = fmaf(w[j], a2.w, T[11]);
+  }
+}
+
 __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
   __shared__ __align__(16) float s_pm[NK][HG];        // pose-map / beta coefficients, [k][hand]
   __shared__ __align__(16) float s_A[HG][16][12];     // skinning transforms (rest pose removed)
@@ -200,82 +336,8 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
       }
       s_pc[h] = pc;
     }
-    float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    float J[3] = {0, 0, 0};
-    if (valid) {
-      const float* m = p.model[side];
-      const float* ps = p.poses + (size_t)hand * 48 + j * 3;
-      float ax = ps[0] + m[OFF_HM + j * 3 + 0];
-      float ay = ps[1] + m[OFF_HM + j * 3 + 1];
-      float az = ps[2] + m[OFF_HM + j * 3 + 2];
-      rodrigues(ax, ay, az, R);
-      const float* b = p.betas + (size_t)hand * 10;
-#pragma unroll
-      for (int c = 0; c < 3; ++c) {
-        float a = m[OFF_JT + j * 3 + c];
-        const float* js = m + OFF_JS + (j * 3 + c) * 10;
-#pragma unroll
-        for (int k = 0; k < 10; ++k) a = fmaf(js[k], b[k], a);
-        J[c] = a;
-      }
-      if (j < 10) s_pm[135 + j][h] = b[j];
-    } else if (j < 10) {
-      s_pm[135 + j][h] = 0.f;
-    }
-#pragma unroll
-    for (int e = 0; e < 9; ++e) s_R[h][j][e] = R[e];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) s_J[h][j][c] = J[c];
-    if (j >= 1) {
-#pragma unroll
-      for (int e = 0; e < 9; ++e) s_pm[(j - 1) * 9 + e][h] = valid ? R[e] - ((e & 3) == 0 ? 1.f : 0.f) : 0.f;
-    }
-    __syncthreads();
-    // kinematic chain: thread j<5 walks finger j (joints 3j+1..3j+3); thread j==5 stores the root
-    if (j <= 5) {
-      float G[12];
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-        G[r * 4 + 0] = s_R[h][0][r * 3 + 0]; G[r * 4 + 1] = s_R[h][0][r * 3 + 1];
-        G[r * 4 + 2] = s_R[h][0][r * 3 + 2]; G[r * 4 + 3] = s_J[h][0][r];
-      }
-      if (j == 5) {
-#pragma unroll
-        for (int e = 0; e < 12; ++e) s_G[h][0][e] = G[e];
-      } else {
-        int parent = 0;
-#pragma unroll
-        for (int lev = 0; lev < 3; ++lev) {
-          const int idx = 3 * j + 1 + lev;
-          const float* Rl = s_R[h][idx];
-          float rel[3] = {s_J[h][idx][0] - s_J[h][parent][0], s_J[h][idx][1] - s_J[h][parent][1],
-                          s_J[h][idx][2] - s_J[h][parent][2]};
-          float N[12];
-#pragma unroll
-          for (int r = 0; r < 3; ++r) {
-#pragma unroll
-            for (int c = 0; c < 3; ++c)
-              N[r * 4 + c] = G[r * 4 + 0] * Rl[0 * 3 + c] + G[r * 4 + 1] * Rl[1 * 3 + c] + G[r * 4 + 2] * Rl[2 * 3 + c];
-            N[r * 4 + 3] = G[r * 4 + 0] * rel[0] + G[r * 4 + 1] * rel[1] + G[r * 4 + 2] * rel[2] + G[r * 4 + 3];
-          }
-#pragma unroll
-          for (int e = 0; e < 12; ++e) { G[e] = N[e]; s_G[h][idx][e] = N[e]; }
-          parent = idx;
-        }
-      }
-    }
-    __syncthreads();
-    // A_j = [R_g | t_g - R_g . J_j]   (manolayer.py:226-228)
-    {
-      const float* G = s_G[h][j];
-#pragma unroll
-      for (int r = 0; r < 3; ++r) {
-        s_A[h][j][r * 4 + 0] = G[r * 4 + 0]; s_A[h][j][r * 4 + 1] = G[r * 4 + 1]; s_A[h][j][r * 4 + 2] = G[r * 4 + 2];
-        s_A[h][j][r * 4 + 3] = G[r * 4 + 3] - (G[r * 4 + 0] * J[0] + G[r * 4 + 1] * J[1] + G[r * 4 + 2] * J[2]);
-      }
-    }
-    if (j < 3) s_ctr[h][j] = (p.center_src >= 0) ? s_G[h][p.center_src][j * 4 + 3] : 0.f;
-    __syncthreads();
+    rebuild_transforms(valid, p.model[valid ? side : 0], p.poses, p.betas, hand, h, j, p.center_src, s_pm, s_A, s_R,
+                       s_J, s_G, s_ctr);
     // kinematic joints + centre are written once per hand group (vertex chunk 0)
     if (blockIdx.y == 0 && valid) {
       const float* G = s_G[h][j];
@@ -294,36 +356,8 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
     for (int h = 0; h < HG; ++h) any |= (s_side[h] == side);
     if (!any) continue;  // block-uniform
     const float* __restrict__ m = p.model[side];
-    const float* __restrict__ dirs = m + OFF_DIRS;
-    unsigned long long acc2[HG / 2][3];   // (hand 2i, hand 2i+1) packed: one ffma2 (two fp32 FMAs) serves two hands
-    {
-      const float v0 = m[OFF_VT + 0 * NVP + vc], v1 = m[OFF_VT + 1 * NVP + vc], v2 = m[OFF_VT + 2 * NVP + vc];
-#pragma unroll
-      for (int h = 0; h < HG / 2; ++h) { acc2[h][0] = pk2(v0, v0); acc2[h][1] = pk2(v1, v1); acc2[h][2] = pk2(v2, v2); }
-    }
-    // shape rows first (v_shaped), then pose rows, like the reference's evaluation order
-#pragma unroll 5
-    for (int kk = 0; kk < NK; ++kk) {
-      const int k = (kk < 10) ? 135 + kk : kk - 10;
-      const float d0 = __ldg(dirs + ((size_t)k * 3 + 0) * NVP + vc);
-      const float d1 = __ldg(dirs + ((size_t)k * 3 + 1) * NVP + vc);
-      const float d2 = __ldg(dirs + ((size_t)k * 3 + 2) * NVP + vc);
-      const float4 pa = *reinterpret_cast<const float4*>(&s_pm[k][0]);
-      const float4 pb = *reinterpret_cast<const float4*>(&s_pm[k][4]);
-      const unsigned long long D0 = pk2(d0, d0), D1 = pk2(d1, d1), D2 = pk2(d2, d2);
-      const unsigned long long P[4] = {pk2(pa.x, pa.y), pk2(pa.z, pa.w), pk2(pb.x, pb.y), pk2(pb.z, pb.w)};
-#pragma unroll
-      for (int h = 0; h < HG / 2; ++h) {
-        ffma2(acc2[h][0], D0, P[h]);
-        ffma2(acc2[h][1], D1, P[h]);
-        ffma2(acc2[h][2], D2, P[h]);
-      }
-    }
     float acc[HG][3];
-#pragma unroll
-    for (int h = 0; h < HG / 2; ++h)
-#pragma unroll
-      for (int c = 0; c < 3; ++c) unpk2(acc2[h][c], acc[2 * h][c], acc[2 * h + 1][c]);
+    blend_vertex(m, vc, s_pm, acc);
     float w[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) w[j] = __ldg(m + OFF_W + j * NVP + vc);
@@ -335,17 +369,7 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
     for (int h = 0; h < HG; ++h) {
       if (s_side[h] != side) continue;  // block-uniform
       float T[12];
-#pragma unroll
-      for (int e = 0; e < 12; ++e) T[e] = 0.f;
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const float4 a0 = *reinterpret_cast<const float4*>(&s_A[h][j][0]);
-        const float4 a1 = *reinterpret_cast<const float4*>(&s_A[h][j][4]);
-        const float4 a2 = *reinterpret_cast<const float4*>(&s_A[h][j][8]);
-        T[0] = fmaf(w[j], a0.x, T[0]); T[1] = fmaf(w[j], a0.y, T[1]); T[2] = fmaf(w[j], a0.z, T[2]); T[3] = fmaf(w[j], a0.w, T[3]);
-        T[4] = fmaf(w[j], a1.x, T[4]); T[5] = fmaf(w[j], a1.y, T[5]); T[6] = fmaf(w[j], a1.z, T[6]); T[7] = fmaf(w[j], a1.w, T[7]);
-        T[8] = fmaf(w[j], a2.x, T[8]); T[9] = fmaf(w[j], a2.y, T[9]); T[10] = fmaf(w[j], a2.z, T[10]); T[11] = fmaf(w[j], a2.w, T[11]);
-      }
+      skin_transform(w, s_A[h], T);
       const float x = T[0] * acc[h][0] + T[1] * acc[h][1] + T[2] * acc[h][2] + T[3] - s_ctr[h][0];
       const float y = T[4] * acc[h][0] + T[5] * acc[h][1] + T[6] * acc[h][2] + T[7] - s_ctr[h][1];
       const float z = T[8] * acc[h][0] + T[9] * acc[h][1] + T[10] * acc[h][2] + T[11] - s_ctr[h][2];
@@ -492,6 +516,327 @@ __global__ void rot6d_to_aa_kernel(const float* __restrict__ r6, int n, float* _
   aa[i * 3 + 0] = o[0]; aa[i * 3 + 1] = o[1]; aa[i * 3 + 2] = o[2];
 }
 
+// ------------------------------------------------------------------------------------------------- MANO backward
+// Two launches, no atomics, nothing saved from the forward.
+//   vertex kernel (forward grid): rebuild phase 1, recompute v_posed and the skinning transform T of every vertex,
+//     take its cotangent du (dverts + the joint cotangent of a fingertip) and reduce, per CTA and hand,
+//       dA_j = sum_v w_vj [du v_posed^T | du]        (16 x 3x4)
+//       dpm_k = sum_v dirs_k . (T[:, :3]^T du)       (145 blend-row coefficients)
+//       sum_v du                                     (for the centre)
+//     into the caller's workspace, one fixed-order partial per (hand, vertex chunk).
+//   chain kernel (one CTA per HG hands, thread = (hand, joint)): sum the partials over the chunks in order, run the
+//     A_j and chain backward (tips to root), Rodrigues backward, and the J_regressor . shapedirs term of dbetas.
+constexpr int NCHUNK = (NV + VPB - 1) / VPB;   // vertex chunks per hand
+constexpr int WS_DA = 0, WS_DPM = 192, WS_DU = WS_DPM + NK, WS_STRIDE = WS_DU + 3;   // floats per (hand, chunk)
+constexpr int DUVP_STRIDE = VPB * 6 + 2;       // per hand: (du, v_posed) of every vertex; +2 spreads the banks
+
+struct ManoGradParams {
+  const float* model;
+  int side;
+  const float* poses;
+  const float* betas;
+  int n;
+  int center_src;
+  const float* dverts;
+  const float* djoints;
+  const float* dcenter;
+  float* ws;
+  int have_partials;   // 0: no vertex / joint cotangent, the vertex kernel did not run
+  float* dposes;
+  float* dbetas;
+};
+
+constexpr size_t GRAD_DYN_SMEM = (size_t)(HG * DUVP_STRIDE + 3 * VPB * HG + 3 * NK * HG) * sizeof(float);
+
+__global__ void __launch_bounds__(VPB) mano_backward_vertex_kernel(const ManoGradParams p) {
+  __shared__ __align__(16) float s_pm[NK][HG];
+  __shared__ __align__(16) float s_A[HG][16][12];
+  __shared__ float s_R[HG][16][9];
+  __shared__ float s_J[HG][16][3];
+  __shared__ float s_G[HG][16][12];
+  __shared__ float s_ctr[HG][3];
+  extern __shared__ __align__(16) float s_dyn[];
+  float* s_duvp = s_dyn;                        // [HG][DUVP_STRIDE]
+  float* s_dvp = s_duvp + HG * DUVP_STRIDE;     // [3][VPB][HG]   d v_posed
+  float* s_dpm3 = s_dvp + 3 * VPB * HG;         // [3][NK][HG]    dpm per coordinate
+
+  const int g0 = blockIdx.x * HG;
+  const int t = threadIdx.x;
+  const float* __restrict__ m = p.model;
+  {
+    const int h = t >> 4, j = t & 15;
+    rebuild_transforms<true>(g0 + h < p.n, m, p.poses, p.betas, g0 + h, h, j, p.center_src, s_pm, s_A, s_R, s_J, s_G, s_ctr);
+  }
+  const int v0 = blockIdx.y * VPB;
+  const int nv = min(VPB, NV - v0);
+  // ---- per vertex: du, v_posed and d v_posed = T[:, :3]^T du of every hand
+  {
+    const int v = v0 + t;
+    const bool vvalid = v < NV;
+    const int vc = vvalid ? v : NVP - 1;
+    float acc[HG][3];
+    blend_vertex(m, vc, s_pm, acc);
+    float w[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) w[j] = __ldg(m + OFF_W + j * NVP + vc);
+    int tip = -1;
+    if (v == 745) tip = 0; else if (v == 317) tip = 1; else if (v == (p.side ? 444 : 445)) tip = 2;
+    else if (v == 556) tip = 3; else if (v == 673) tip = 4;
+#pragma unroll
+    for (int h = 0; h < HG; ++h) {
+      const int hand = g0 + h;
+      float du[3] = {0.f, 0.f, 0.f};
+      if (vvalid && hand < p.n) {
+        if (p.dverts) {
+          const float* d = p.dverts + ((size_t)hand * NV + v) * 3;
+          du[0] = d[0]; du[1] = d[1]; du[2] = d[2];
+        }
+        if (tip >= 0 && p.djoints) {
+          const float* d = p.djoints + ((size_t)hand * 21 + c_joint_inv[16 + tip]) * 3;
+          du[0] += d[0]; du[1] += d[1]; du[2] += d[2];
+        }
+      }
+      float T[12];
+      skin_transform(w, s_A[h], T);
+      float* o = s_duvp + h * DUVP_STRIDE + t * 6;
+      o[0] = du[0]; o[1] = du[1]; o[2] = du[2]; o[3] = acc[h][0]; o[4] = acc[h][1]; o[5] = acc[h][2];
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        s_dvp[(c * VPB + t) * HG + h] = T[0 * 4 + c] * du[0] + T[1 * 4 + c] * du[1] + T[2 * 4 + c] * du[2];
+    }
+  }
+  __syncthreads();
+  // ---- dA_j and sum(du): thread (h, j), vertices in order
+  {
+    const int h = t >> 4, j = t & 15;
+    const float* __restrict__ wj = m + OFF_W + (size_t)j * NVP + v0;
+    const float* d = s_duvp + h * DUVP_STRIDE;
+    float a[12], su[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int e = 0; e < 12; ++e) a[e] = 0.f;
+    for (int i = 0; i < nv; ++i) {
+      const float wv = __ldg(wj + i);
+      const float2 q0 = *reinterpret_cast<const float2*>(d + 6 * i);
+      const float2 q1 = *reinterpret_cast<const float2*>(d + 6 * i + 2);
+      const float2 q2 = *reinterpret_cast<const float2*>(d + 6 * i + 4);
+      const float du[3] = {q0.x, q0.y, q1.x}, vp[3] = {q1.y, q2.x, q2.y};
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+        const float wd = wv * du[r];
+        a[r * 4 + 0] = fmaf(wd, vp[0], a[r * 4 + 0]);
+        a[r * 4 + 1] = fmaf(wd, vp[1], a[r * 4 + 1]);
+        a[r * 4 + 2] = fmaf(wd, vp[2], a[r * 4 + 2]);
+        a[r * 4 + 3] += wd;
+        su[r] += du[r];
+      }
+    }
+    const int hand = g0 + h;
+    if (hand < p.n) {
+      float* o = p.ws + ((size_t)hand * NCHUNK + blockIdx.y) * WS_STRIDE;
+#pragma unroll
+      for (int e = 0; e < 12; ++e) o[WS_DA + j * 12 + e] = a[e];
+      if (j == 0) { o[WS_DU + 0] = su[0]; o[WS_DU + 1] = su[1]; o[WS_DU + 2] = su[2]; }
+    }
+  }
+  // ---- dpm per (coordinate, row): the row is streamed from L2 (16-byte loads; the model's zero padding and the
+  //      zero cotangent of the tail threads cover the rounded-up length), the HG cotangents are broadcast
+  {
+    const int nv4 = (nv + 3) & ~3;
+    for (int task = t; task < 3 * NK; task += VPB) {
+      const int c = task / NK, k = task - c * NK;
+      const float* __restrict__ dr = m + OFF_DIRS + ((size_t)k * 3 + c) * NVP + v0;
+      const float* dv = s_dvp + c * VPB * HG;
+      float s[HG];
+#pragma unroll
+      for (int h = 0; h < HG; ++h) s[h] = 0.f;
+      for (int i = 0; i < nv4; i += 4) {
+        const float4 d4 = __ldg(reinterpret_cast<const float4*>(dr + i));
+        const float dd[4] = {d4.x, d4.y, d4.z, d4.w};
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          const float4 x0 = *reinterpret_cast<const float4*>(dv + (i + u) * HG);
+          const float4 x1 = *reinterpret_cast<const float4*>(dv + (i + u) * HG + 4);
+          s[0] = fmaf(dd[u], x0.x, s[0]); s[1] = fmaf(dd[u], x0.y, s[1]);
+          s[2] = fmaf(dd[u], x0.z, s[2]); s[3] = fmaf(dd[u], x0.w, s[3]);
+          s[4] = fmaf(dd[u], x1.x, s[4]); s[5] = fmaf(dd[u], x1.y, s[5]);
+          s[6] = fmaf(dd[u], x1.z, s[6]); s[7] = fmaf(dd[u], x1.w, s[7]);
+        }
+      }
+      float4* o = reinterpret_cast<float4*>(s_dpm3 + (c * NK + k) * HG);
+      o[0] = make_float4(s[0], s[1], s[2], s[3]);
+      o[1] = make_float4(s[4], s[5], s[6], s[7]);
+    }
+  }
+  __syncthreads();
+  for (int task = t; task < NK * HG; task += VPB) {
+    const int h = task / NK, k = task - h * NK;
+    const int hand = g0 + h;
+    if (hand >= p.n) continue;
+    const float v = s_dpm3[(0 * NK + k) * HG + h] + s_dpm3[(1 * NK + k) * HG + h] + s_dpm3[(2 * NK + k) * HG + h];
+    p.ws[((size_t)hand * NCHUNK + blockIdx.y) * WS_STRIDE + WS_DPM + k] = v;
+  }
+}
+
+__global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGradParams p) {
+  __shared__ __align__(16) float s_pm[NK][HG];
+  __shared__ __align__(16) float s_A[HG][16][12];
+  __shared__ float s_R[HG][16][9];
+  __shared__ float s_J[HG][16][3];
+  __shared__ float s_G[HG][16][12];
+  __shared__ float s_ctr[HG][3];
+  __shared__ float s_dG[HG][16][12];     // cotangent of the global transforms [R_g | t_g]
+  __shared__ float s_dJ[HG][16][3];      // cotangent of the rest joints
+  __shared__ float s_dR[HG][16][9];      // cotangent of the local rotations (chain part)
+  __shared__ float s_root[HG][5][15];    // per finger: its level-1 contribution to dG_0 (12) and dJ_0 (3)
+  __shared__ float s_dctr[HG][3];
+
+  const int t = threadIdx.x, h = t >> 4, j = t & 15;
+  const int hand = blockIdx.x * HG + h;
+  const bool valid = hand < p.n;
+  rebuild_transforms<true>(valid, p.model, p.poses, p.betas, hand, h, j, p.center_src, s_pm, s_A, s_R, s_J, s_G, s_ctr);
+  const float* __restrict__ m = p.model;
+  // ---- partials of the vertex kernel, summed over the chunks in order
+  float dA[12], dpm[9], dpb = 0.f;
+#pragma unroll
+  for (int e = 0; e < 12; ++e) dA[e] = 0.f;
+#pragma unroll
+  for (int e = 0; e < 9; ++e) dpm[e] = 0.f;
+  if (valid && p.have_partials) {
+    for (int ch = 0; ch < NCHUNK; ++ch) {
+      const float* w = p.ws + ((size_t)hand * NCHUNK + ch) * WS_STRIDE;
+#pragma unroll
+      for (int e = 0; e < 12; ++e) dA[e] += w[WS_DA + j * 12 + e];
+      if (j >= 1) {
+#pragma unroll
+        for (int e = 0; e < 9; ++e) dpm[e] += w[WS_DPM + (j - 1) * 9 + e];
+      }
+      if (j < 10) dpb += w[WS_DPM + 135 + j];
+    }
+  }
+  // ---- centre: d ctr = dcenter - sum(dverts) - sum(djoints)  (every output had the centre subtracted)
+  if (j < 3) {
+    float d = 0.f;
+    if (valid && p.center_src >= 0) {
+      if (p.dcenter) d = p.dcenter[(size_t)hand * 3 + j];
+      if (p.have_partials)   // sum of du = dverts + fingertip joint cotangents
+        for (int ch = 0; ch < NCHUNK; ++ch) d -= p.ws[((size_t)hand * NCHUNK + ch) * WS_STRIDE + WS_DU + j];
+      if (p.djoints)
+        for (int s = 0; s < 16; ++s) d -= p.djoints[((size_t)hand * 21 + c_joint_inv[s]) * 3 + j];
+    }
+    s_dctr[h][j] = d;
+  }
+  __syncthreads();
+  // ---- A_j = [R_g | t_g - R_g J_j]  and the kinematic joint outputs t_g (- ctr)
+  {
+    const float* G = s_G[h][j];
+    float dt[3] = {0.f, 0.f, 0.f};
+    if (valid && p.djoints) {
+      const float* d = p.djoints + ((size_t)hand * 21 + c_joint_inv[j]) * 3;
+      dt[0] = d[0]; dt[1] = d[1]; dt[2] = d[2];
+    }
+    if (j == p.center_src) { dt[0] += s_dctr[h][0]; dt[1] += s_dctr[h][1]; dt[2] += s_dctr[h][2]; }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s_dG[h][j][r * 4 + c] = dA[r * 4 + c] - dA[r * 4 + 3] * s_J[h][j][c];
+      s_dG[h][j][r * 4 + 3] = dt[r] + dA[r * 4 + 3];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      s_dJ[h][j][c] = -(G[0 * 4 + c] * dA[0 * 4 + 3] + G[1 * 4 + c] * dA[1 * 4 + 3] + G[2 * 4 + c] * dA[2 * 4 + 3]);
+  }
+  __syncthreads();
+  // ---- chain backward: thread j<5 walks finger j from the tip to the root
+  if (j < 5) {
+    float dN[12];
+#pragma unroll
+    for (int e = 0; e < 12; ++e) dN[e] = s_dG[h][3 * j + 3][e];
+#pragma unroll
+    for (int lev = 2; lev >= 0; --lev) {
+      const int idx = 3 * j + 1 + lev, parent = lev ? idx - 1 : 0;
+      const float* Gp = s_G[h][parent];
+      const float* Rl = s_R[h][idx];
+      const float rel[3] = {s_J[h][idx][0] - s_J[h][parent][0], s_J[h][idx][1] - s_J[h][parent][1],
+                            s_J[h][idx][2] - s_J[h][parent][2]};
+      // N = Gp [Rl | rel] + [0 | t_p]:  dRl = Gp^T dN[:, :3], drel = Gp^T dN[:, 3]
+#pragma unroll
+      for (int i = 0; i < 3; ++i) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+          s_dR[h][idx][i * 3 + c] = Gp[0 * 4 + i] * dN[0 * 4 + c] + Gp[1 * 4 + i] * dN[1 * 4 + c] + Gp[2 * 4 + i] * dN[2 * 4 + c];
+      }
+      float drel[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) drel[i] = Gp[0 * 4 + i] * dN[0 * 4 + 3] + Gp[1 * 4 + i] * dN[1 * 4 + 3] + Gp[2 * 4 + i] * dN[2 * 4 + 3];
+      // dGp[:, :3] = dN[:, :3] Rl^T + dN[:, 3] rel^T,  dGp[:, 3] = dN[:, 3]
+      float dP[12];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int i = 0; i < 3; ++i)
+          dP[r * 4 + i] = dN[r * 4 + 0] * Rl[i * 3 + 0] + dN[r * 4 + 1] * Rl[i * 3 + 1] + dN[r * 4 + 2] * Rl[i * 3 + 2] +
+                          dN[r * 4 + 3] * rel[i];
+        dP[r * 4 + 3] = dN[r * 4 + 3];
+      }
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s_dJ[h][idx][c] += drel[c];
+      if (lev) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) s_dJ[h][parent][c] -= drel[c];
+#pragma unroll
+        for (int e = 0; e < 12; ++e) dN[e] = s_dG[h][parent][e] + dP[e];
+      } else {
+#pragma unroll
+        for (int e = 0; e < 12; ++e) s_root[h][j][e] = dP[e];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) s_root[h][j][12 + c] = -drel[c];
+      }
+    }
+  }
+  __syncthreads();
+  // ---- root G_0 = [R_0 | J_0]: the five fingers' contributions in order
+  if (j == 0) {
+    float dG0[12], dJ0[3];
+#pragma unroll
+    for (int e = 0; e < 12; ++e) dG0[e] = s_dG[h][0][e];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) dJ0[c] = s_dJ[h][0][c];
+    for (int f = 0; f < 5; ++f) {
+#pragma unroll
+      for (int e = 0; e < 12; ++e) dG0[e] += s_root[h][f][e];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) dJ0[c] += s_root[h][f][12 + c];
+    }
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s_dR[h][0][r * 3 + c] = dG0[r * 4 + c];
+      s_dJ[h][0][r] = dJ0[r] + dG0[r * 4 + 3];
+    }
+  }
+  __syncthreads();
+  if (!valid) return;
+  // ---- Rodrigues backward (pose map = R - I for joints 1..15)
+  if (p.dposes) {
+    float g[9];
+#pragma unroll
+    for (int e = 0; e < 9; ++e) g[e] = s_dR[h][j][e] + dpm[e];
+    const float* ps = p.poses + (size_t)hand * 48 + j * 3;
+    float da[3];
+    rodrigues_vjp(ps[0] + m[OFF_HM + j * 3 + 0], ps[1] + m[OFF_HM + j * 3 + 1], ps[2] + m[OFF_HM + j * 3 + 2], g, da);
+    float* o = p.dposes + (size_t)hand * 48 + j * 3;
+    o[0] = da[0]; o[1] = da[1]; o[2] = da[2];
+  }
+  // ---- betas: the shape rows of the vertices plus J = JT + JS . beta
+  if (p.dbetas && j < 10) {
+    float d = dpb;
+    for (int s = 0; s < 16; ++s)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) d = fmaf(m[OFF_JS + (s * 3 + c) * 10 + j], s_dJ[h][s][c], d);
+    p.dbetas[(size_t)hand * 10 + j] = d;
+  }
+}
+
 }  // namespace acr
 
 using namespace acr;
@@ -608,6 +953,46 @@ extern "C" int acr_b200_mano_forward_gather(const float* model_l, const float* m
   ACR_CHECK_ARG(gather != nullptr, "mano_forward_gather: gather descriptor is null");
   return mano_forward_impl(model_l, model_r, poses, betas, hand_type, default_side, n_dev, n_max, center_idx, cam,
                            offsets, verts, joints, center, verts_camed, pj2d, pj2d_org, counts_src, gather, stream);
+}
+
+extern "C" size_t acr_b200_mano_backward_workspace_floats(int n) {
+  return n > 0 ? (size_t)n * NCHUNK * WS_STRIDE : 0;
+}
+
+extern "C" int acr_b200_mano_backward(const float* model, int side, const float* poses, const float* betas, int n,
+                                      int center_idx, const float* dverts, const float* djoints, const float* dcenter,
+                                      float* workspace, float* dposes, float* dbetas, void* stream) {
+  ACR_CHECK_ARG(n >= 0, "mano_backward: n < 0");
+  if (n == 0) return ACR_B200_OK;
+  ACR_CHECK_ARG(model && poses && betas, "mano_backward: model / poses / betas are null");
+  ACR_CHECK_ARG(side == 0 || side == 1, "mano_backward: side must be 0 (left) or 1 (right)");
+  ACR_CHECK_ARG(center_idx >= -1 && center_idx < 21, "mano_backward: center_idx out of range");
+  const bool partials = dverts || djoints;
+  ACR_CHECK_ARG(!partials || workspace, "mano_backward: workspace is null (acr_b200_mano_backward_workspace_floats)");
+  static const int perm[21] = {0, 13, 14, 15, 16, 1, 2, 3, 17, 4, 5, 6, 18, 10, 11, 12, 19, 7, 8, 9, 20};
+  int center_src = -1;
+  if (center_idx >= 0) {
+    center_src = perm[center_idx];
+    if (center_src >= 16) {
+      set_error("mano_backward: centring on a fingertip joint (center_idx=%d) is not supported", center_idx);
+      return ACR_B200_ENOTSUP;
+    }
+  }
+  if (!dposes && !dbetas) return ACR_B200_OK;
+  ManoGradParams p = {};
+  p.model = model; p.side = side; p.poses = poses; p.betas = betas; p.n = n; p.center_src = center_src;
+  p.dverts = dverts; p.djoints = djoints; p.dcenter = dcenter; p.ws = workspace; p.have_partials = partials;
+  p.dposes = dposes; p.dbetas = dbetas;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (partials) {
+    static unsigned long long smem_done = 0;
+    ACR_CHECK_CUDA(ensure_dynamic_smem(mano_backward_vertex_kernel, (int)GRAD_DYN_SMEM, &smem_done));
+    mano_backward_vertex_kernel<<<dim3(ceil_div(n, HG), NCHUNK), VPB, GRAD_DYN_SMEM, s>>>(p);
+    ACR_CHECK_LAUNCH();
+  }
+  mano_backward_chain_kernel<<<ceil_div(n, HG), VPB, 0, s>>>(p);
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
 }
 
 extern "C" int acr_b200_gather_wait(const acr_b200_gather* g, void* stream) {

@@ -15,13 +15,22 @@ __device__ __forceinline__ float dot3_rn(float ax, float ay, float az, float bx,
   return __fadd_rn(__fadd_rn(__fmul_rn(ax, bx), __fmul_rn(ay, by)), __fmul_rn(az, bz));
 }
 
+// sin / cos of half the rotation angle.  kPiTrig selects sincospif, whose argument reduction is exact and needs no
+// local memory (sincosf's large-argument path keeps a scratch array there); the two agree to an ulp or two.
+template <bool kPiTrig>
+__device__ __forceinline__ void half_angle_sincos(float ang, float* s, float* c) {
+  if constexpr (kPiTrig) sincospif(ang * 0.159154943f, s, c);   // ang / (2 pi)
+  else sincosf(ang * 0.5f, s, c);
+}
+
+template <bool kPiTrig = false>
 __device__ __forceinline__ void rodrigues(float ax, float ay, float az, float* R) {
   // angle = || aa + 1e-8 ||, axis = aa / angle, q = [cos(a/2), sin(a/2) axis], q /= ||q||
   const float bx = ax + 1e-8f, by = ay + 1e-8f, bz = az + 1e-8f;
   const float ang = sqrtf(bx * bx + by * by + bz * bz);
   const float nx = ax / ang, ny = ay / ang, nz = az / ang;
   float s, c;
-  sincosf(ang * 0.5f, &s, &c);
+  half_angle_sincos<kPiTrig>(ang, &s, &c);
   float w = c, x = s * nx, y = s * ny, z = s * nz;
   const float qn = sqrtf(w * w + x * x + y * y + z * z);
   w /= qn; x /= qn; y /= qn; z /= qn;
@@ -30,6 +39,37 @@ __device__ __forceinline__ void rodrigues(float ax, float ay, float az, float* R
   R[0] = w2 + x2 - y2 - z2; R[1] = 2 * xy - 2 * wz;   R[2] = 2 * wy + 2 * xz;
   R[3] = 2 * wz + 2 * xy;   R[4] = w2 - x2 + y2 - z2; R[5] = 2 * yz - 2 * wx;
   R[6] = 2 * xz - 2 * wy;   R[7] = 2 * wx + 2 * yz;   R[8] = w2 - x2 - y2 + z2;
+}
+
+// Vector-Jacobian product of rodrigues(): dR (row-major 3x3 cotangent) -> da, the exact derivative of the
+// quaternion form above (the 1e-8 offset sits in the angle only, the axis numerator is `a`).  Written in n = a/angle
+// and s/angle = sin(angle/2)/angle, which stay bounded, so it is finite at a = 0 (angle = sqrt(3)*1e-8).
+__device__ __forceinline__ void rodrigues_vjp(float ax, float ay, float az, const float* g, float* da) {
+  const float bx = ax + 1e-8f, by = ay + 1e-8f, bz = az + 1e-8f;
+  const float ang = sqrtf(bx * bx + by * by + bz * bz);
+  const float nx = ax / ang, ny = ay / ang, nz = az / ang;
+  float s, c;
+  half_angle_sincos<true>(ang, &s, &c);
+  const float q[4] = {c, s * nx, s * ny, s * nz};
+  const float qn = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  const float w = q[0] / qn, x = q[1] / qn, y = q[2] / qn, z = q[3] / qn;
+  // quat2mat: d/d(w,x,y,z) of the nine entries, contracted with g
+  float dq[4];
+  dq[0] = 2.f * (w * (g[0] + g[4] + g[8]) + x * (g[7] - g[5]) + y * (g[2] - g[6]) + z * (g[3] - g[1]));
+  dq[1] = 2.f * (x * (g[0] - g[4] - g[8]) + y * (g[1] + g[3]) + z * (g[2] + g[6]) + w * (g[7] - g[5]));
+  dq[2] = 2.f * (y * (g[4] - g[0] - g[8]) + x * (g[1] + g[3]) + w * (g[2] - g[6]) + z * (g[5] + g[7]));
+  dq[3] = 2.f * (z * (g[8] - g[0] - g[4]) + w * (g[3] - g[1]) + x * (g[2] + g[6]) + y * (g[5] + g[7]));
+  // q / ||q||
+  const float proj = w * dq[0] + x * dq[1] + y * dq[2] + z * dq[3];
+  dq[0] = (dq[0] - w * proj) / qn; dq[1] = (dq[1] - x * proj) / qn;
+  dq[2] = (dq[2] - y * proj) / qn; dq[3] = (dq[3] - z * proj) / qn;
+  // q = [cos(ang/2), sin(ang/2) a/ang], ang = ||a + 1e-8||
+  const float sa = s / ang;
+  const float nd = nx * dq[1] + ny * dq[2] + nz * dq[3];
+  const float dang = 0.5f * (c * nd - s * dq[0]) - sa * nd;
+  da[0] = sa * dq[1] + dang * (bx / ang);
+  da[1] = sa * dq[2] + dang * (by / ang);
+  da[2] = sa * dq[3] + dang * (bz / ang);
 }
 
 // rotation_matrix_to_angle_axis (acr/utils.py:334-360) of a row-major 3x3 (not necessarily orthonormal)

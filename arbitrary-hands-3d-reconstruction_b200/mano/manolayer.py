@@ -3,6 +3,10 @@
 Mirrors the constructor, buffers and ``forward`` signature of the reference
 (/root/reference/mano/manolayer.py:13-22, :65-93, :104-110, :273-276); the ~124 ATen launches of
 the reference forward (:104-276) become a single ``acr_b200_mano_forward`` call.
+
+The layer is differentiable with respect to the pose (or PCA coefficients), betas and ``th_trans``: with grad
+enabled and pose or betas requiring grad, the kernel runs inside ``_ManoFunction``, whose backward is the fused
+``acr_b200_mano_backward``.  Otherwise the forward makes exactly the launch it makes without autograd.
 """
 from __future__ import annotations
 
@@ -10,12 +14,40 @@ from typing import Optional
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 from torch.nn import Module
 
 from acr_b200 import ops as _ops
 from mano.assets import get_asset
 
 _ZERO1 = torch.zeros(1)
+
+
+class _ManoFunction(torch.autograd.Function):
+    """(pose (n,48) without the mean pose, betas (n,10)) -> (verts, joints, center) of one side; the backward is the
+    fused MANO backward kernel (first order only)."""
+
+    @staticmethod
+    def forward(ctx, pose, betas, model, side, center_idx):
+        out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose, betas, None, side,
+                                center_idx)
+        ctx.save_for_backward(pose, betas)
+        ctx.model, ctx.side, ctx.center_idx = model, side, center_idx
+        ctx.set_materialize_grads(False)     # an unused output's cotangent stays None and reaches the kernel as NULL
+        return out["verts"], out["joints"], out["center"]
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dverts, djoints, dcenter):
+        pose, betas = ctx.saved_tensors
+        want_pose, want_betas = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        if ctx.center_idx is None:
+            dcenter = None                   # the centre output is zero and does not depend on the inputs
+        if dverts is None and djoints is None and dcenter is None:
+            return None, None, None, None, None
+        dpose, dbetas = _ops.mano_backward(ctx.model, ctx.side, pose, betas, ctx.center_idx, dverts, djoints, dcenter,
+                                           want_pose, want_betas)
+        return dpose, dbetas, None, None, None
 
 
 class ManoLayer(Module):
@@ -73,7 +105,6 @@ class ManoLayer(Module):
             self._packed_key = key
         return self._packed
 
-    @torch.no_grad()
     def forward(self, th_pose_coeffs, th_betas=_ZERO1, th_trans=_ZERO1, root_palm=torch.Tensor([0]),
                 share_betas=torch.Tensor([0])):
         if bool(root_palm):
@@ -92,13 +123,16 @@ class ManoLayer(Module):
         center_idx = None if use_trans else self.center_idx
         side = 1 if self.side == 'right' else 0
         model = self.packed_model()
-        out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose[:, :48],
-                                betas, None, side, center_idx)
-        verts, jtr = out["verts"], out["joints"]
+        if torch.is_grad_enabled() and (pose.requires_grad or betas.requires_grad):
+            verts, jtr, center = _ManoFunction.apply(pose[:, :48], betas, model, side, center_idx)
+        else:
+            out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose[:, :48],
+                                    betas, None, side, center_idx)
+            verts, jtr, center = out["verts"], out["joints"], out["center"]
         if use_trans:
             verts = verts + th_trans.unsqueeze(1)
             jtr = jtr + th_trans.unsqueeze(1)
             return verts, jtr, th_trans.unsqueeze(1)
         if self.center_idx is None:
             return verts, jtr, None
-        return verts, jtr, out["center"]
+        return verts, jtr, center

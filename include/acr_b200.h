@@ -107,6 +107,23 @@ int acr_b200_mano_forward_gather(const float* model_l, const float* model_r, con
 /* Stream-ordered wait until the most recent gather launch of EVERY rank has landed in this rank's buffer. */
 int acr_b200_gather_wait(const acr_b200_gather* gather, void* stream);
 
+/* Backward of acr_b200_mano_forward for one side (the gradient of ManoLayer.forward, mano/manolayer.py:104-276,
+ * which the reference gets from torch autograd): cotangents of verts / joints / center -> dposes, dbetas.
+ *   model : packed model of `side` (0 left, 1 right); poses (n,48) WITHOUT the mean pose and betas (n,10): the
+ *           values the forward saw.  Nothing is saved from the forward; the transforms are recomputed.
+ *   center_idx : as in the forward (-1 none; a fingertip is ACR_B200_ENOTSUP).  With a centre, every vertex and
+ *           joint had it subtracted and the centre is itself an output: d centre = dcenter - sum dverts - sum djoints.
+ *   dverts (n,778,3), djoints (n,21,3), dcenter (n,3): cotangents, each may be NULL (= zero).
+ *   workspace : acr_b200_mano_backward_workspace_floats(n) floats of caller-owned device scratch (per hand and
+ *           vertex chunk: partial sums of the skinning-transform and blend-row cotangents); may be NULL when
+ *           dverts and djoints are both NULL.
+ * Outputs dposes (n,48) and dbetas (n,10); either may be NULL (not computed).  fp32; two launches; no atomics,
+ * so repeated calls give bit-identical gradients.                                                      */
+size_t acr_b200_mano_backward_workspace_floats(int n);
+int acr_b200_mano_backward(const float* model, int side, const float* poses, const float* betas, int n,
+                           int center_idx, const float* dverts, const float* djoints, const float* dcenter,
+                           float* workspace, float* dposes, float* dbetas, void* stream);
+
 /* Camera translation of every hand from its 21 joints: the closed-form weighted least squares of
  * estimate_translation_np (acr/utils.py:430-472) -- the reference's own fall-back for the host-side
  * cv2.solvePnPRansac loop (estimate_translation :474-519, called from vertices_kp3d_projection :403-407,
