@@ -97,6 +97,51 @@ def mano_backward(model: torch.Tensor, side: int, poses: torch.Tensor, betas: to
     return dposes, dbetas
 
 
+def mano_layer_forward(model: torch.Tensor, side: int, pose: torch.Tensor, pose_mode: int, betas: torch.Tensor,
+                       center_idx: Optional[int], root_palm: bool):
+    """One side's ManoLayer.forward for any pose input (``L.POSE_AXISANG``: (n,48) without the mean pose;
+    ``L.POSE_ROTMAT``: (n,16,3,3) matrices, projected onto SO(3)) and ``root_palm`` -> (verts, joints, center)."""
+    dev = L.require_cuda(model, pose, betas)
+    n = pose.shape[0]
+    pose = pose.contiguous().float()
+    betas = betas.contiguous().float()
+    verts, joints = torch.empty(n, 778, 3, device=dev), torch.empty(n, 21, 3, device=dev)
+    center = torch.empty(n, 1, 3, device=dev)
+    lib = L.load()
+    with L.on(dev):
+        rc = lib.acr_b200_mano_layer_forward(L.ptr(model), int(side), L.ptr(pose), int(pose_mode), L.ptr(betas), n,
+                                             -1 if center_idx is None else int(center_idx), int(bool(root_palm)),
+                                             L.ptr(verts), L.ptr(joints), L.ptr(center), L.current_stream(dev))
+    L.check(rc, "mano_layer_forward")
+    return verts, joints, center
+
+
+def mano_layer_backward(model: torch.Tensor, side: int, pose: torch.Tensor, pose_mode: int, betas: torch.Tensor,
+                        center_idx: Optional[int], root_palm: bool, dverts: Optional[torch.Tensor],
+                        djoints: Optional[torch.Tensor], dcenter: Optional[torch.Tensor], want_pose: bool = True,
+                        want_betas: bool = True):
+    """Gradient of ``mano_layer_forward`` -> (dpose shaped like pose, dbetas (n,10)); a cotangent of None is zero,
+    an output not wanted comes back as None."""
+    dev = L.require_cuda(model, pose, betas, dverts, djoints, dcenter)
+    n = pose.shape[0]
+    pose = pose.contiguous().float()
+    betas = betas.contiguous().float()
+    dverts, djoints, dcenter = [None if t is None else t.contiguous().float() for t in (dverts, djoints, dcenter)]
+    dpose = torch.empty(pose.shape, device=dev) if want_pose else None
+    dbetas = torch.empty(n, 10, device=dev) if want_betas else None
+    lib = L.load()
+    ws = None
+    if n and (dverts is not None or djoints is not None):
+        ws = torch.empty(int(lib.acr_b200_mano_backward_workspace_floats(n)), device=dev)
+    with L.on(dev):
+        rc = lib.acr_b200_mano_layer_backward(L.ptr(model), int(side), L.ptr(pose), int(pose_mode), L.ptr(betas), n,
+                                              -1 if center_idx is None else int(center_idx), int(bool(root_palm)),
+                                              L.ptr(dverts), L.ptr(djoints), L.ptr(dcenter), L.ptr(ws), L.ptr(dpose),
+                                              L.ptr(dbetas), L.current_stream(dev))
+    L.check(rc, "mano_layer_backward")
+    return dpose, dbetas
+
+
 def cam_trans(j3d: torch.Tensor, pj2d: torch.Tensor, focal_length: float = 1265.0, img_size: float = 512.0,
               n_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(n,21,3), (n,21,2) -> (n,3) camera translation (closed-form least squares on the device)."""

@@ -31,6 +31,12 @@ constexpr size_t OFF_JS = OFF_JT + 48;                      // [16][3][10] J_reg
 constexpr size_t OFF_HM = OFF_JS + 480;                     // [48] 0,0,0, hands_mean
 constexpr size_t MODEL_FLOATS = OFF_HM + 48;
 
+// pose input of the layer entry points (ACR_B200_POSE_* in include/acr_b200.h)
+constexpr int POSE_AXISANG = 0, POSE_ROTMAT = 1;
+// root_palm: output joint 0 is the midpoint of these two vertices (manolayer.py:248-250), both in vertex chunk 0
+constexpr int PALM_VA = 95, PALM_VB = 22;
+static_assert(PALM_VA < VPB && PALM_VB < VPB, "the palm vertices must lie in vertex chunk 0");
+
 // out-joint index of source joint s (inverse of the reference's reorder list, manolayer.py:254)
 __constant__ int c_joint_inv[21] = {0, 5, 6, 7, 9, 10, 11, 17, 18, 19, 13, 14, 15, 1, 2, 3, 4, 8, 12, 16, 20};
 // source joint of out-joint i (the reference's list itself)
@@ -140,7 +146,9 @@ __device__ __forceinline__ void write_joint(const ManoParams& p, int hand, int o
 // fingers (three levels each), and every thread forms its skinning transform A_j.  `m` is the packed model of the
 // hand; a row beyond n (!valid, m unused) gets the identity rotation, a zero joint and zero blend coefficients.
 // Ends synchronised.  kPiTrig as in rodrigues(): the backward kernels use it, so they never touch local memory.
-template <bool kPiTrig = false>
+// kPose: POSE_AXISANG reads (n,48) axis angles (the mean pose is added here); POSE_ROTMAT reads (n,16,3,3) matrices
+// and projects each onto SO(3) like the reference's batch_rotprojs (no mean pose: its rotmat branch has none).
+template <bool kPiTrig = false, int kPose = POSE_AXISANG>
 __device__ __forceinline__ void rebuild_transforms(bool valid, const float* __restrict__ m, const float* __restrict__ poses,
                                                    const float* __restrict__ betas, int hand, int h, int j, int center_src,
                                                    float (*s_pm)[HG], float (*s_A)[16][12], float (*s_R)[16][9],
@@ -148,11 +156,15 @@ __device__ __forceinline__ void rebuild_transforms(bool valid, const float* __re
   float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   float J[3] = {0, 0, 0};
   if (valid) {
-    const float* ps = poses + (size_t)hand * 48 + j * 3;
-    float ax = ps[0] + m[OFF_HM + j * 3 + 0];
-    float ay = ps[1] + m[OFF_HM + j * 3 + 1];
-    float az = ps[2] + m[OFF_HM + j * 3 + 2];
-    rodrigues<kPiTrig>(ax, ay, az, R);
+    if constexpr (kPose == POSE_ROTMAT) {
+      so3_project(poses + ((size_t)hand * 16 + j) * 9, R);
+    } else {
+      const float* ps = poses + (size_t)hand * 48 + j * 3;
+      float ax = ps[0] + m[OFF_HM + j * 3 + 0];
+      float ay = ps[1] + m[OFF_HM + j * 3 + 1];
+      float az = ps[2] + m[OFF_HM + j * 3 + 2];
+      rodrigues<kPiTrig>(ax, ay, az, R);
+    }
     const float* b = betas + (size_t)hand * 10;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -271,7 +283,11 @@ __device__ __forceinline__ void skin_transform(const float (&w)[16], const float
   }
 }
 
-__global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
+// The forward, for the pose input kPose; kPalm replaces output joint 0 (the wrist) by the palm, the midpoint of
+// vertices 95 and 22, which the chunk-0 CTA takes from its staged vertices.
+template <int kPose, bool kPalm>
+__device__ __forceinline__ void mano_forward_body(const ManoParams p) {
+  constexpr bool kGather = kPose == POSE_AXISANG && !kPalm;   // the fused all-gather is compiled into this form only
   __shared__ __align__(16) float s_pm[NK][HG];        // pose-map / beta coefficients, [k][hand]
   __shared__ __align__(16) float s_A[HG][16][12];     // skinning transforms (rest pose removed)
   __shared__ float s_R[HG][16][9];                    // local rotations
@@ -290,7 +306,7 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
   unsigned long long step = 0;
   char* slot_mc = nullptr;
   unsigned long long slot_off = 0;
-  if (p.gather) {
+  if (kGather && p.gather) {
     step = *p.step_dev;                       // stable during the launch: only the last CTA advances it, at the very end
     slot_off = ((step + 1) & 1ull) * p.slot_bytes;
     slot_mc = p.mc_base ? p.mc_base + slot_off : nullptr;
@@ -305,7 +321,7 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
     }
   }
   const bool active = g0 < n;
-  if (active && p.gather) {
+  if (active && kGather && p.gather) {
     // Slot (step+1)&1 was last written by step-1.  A peer signals step `step` only after its launch `step`, which it
     // enqueued after consuming step-1's data (the consume-before-next-launch contract) -> once every peer's flag in
     // OUR memory reads >= step, nobody reads the slot any more.  With two slots this wait is one whole step old.
@@ -336,12 +352,13 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
       }
       s_pc[h] = pc;
     }
-    rebuild_transforms(valid, p.model[valid ? side : 0], p.poses, p.betas, hand, h, j, p.center_src, s_pm, s_A, s_R,
-                       s_J, s_G, s_ctr);
+    rebuild_transforms<false, kPose>(valid, p.model[valid ? side : 0], p.poses, p.betas, hand, h, j, p.center_src, s_pm,
+                                     s_A, s_R, s_J, s_G, s_ctr);
     // kinematic joints + centre are written once per hand group (vertex chunk 0)
     if (blockIdx.y == 0 && valid) {
       const float* G = s_G[h][j];
-      write_joint(p, hand, c_joint_inv[j], G[3] - s_ctr[h][0], G[7] - s_ctr[h][1], G[11] - s_ctr[h][2], s_pc[h]);
+      if (!(kPalm && j == 0))
+        write_joint(p, hand, c_joint_inv[j], G[3] - s_ctr[h][0], G[7] - s_ctr[h][1], G[11] - s_ctr[h][2], s_pc[h]);
       if (j < 3 && p.center) p.center[(size_t)hand * 3 + j] = s_ctr[h][j];
     }
   }
@@ -390,6 +407,15 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
   // 16-byte chunk j of the row IS an aligned 16-byte chunk of global memory: one float4 (or multimem.st.v4 / peer
   // float4) per thread and chunk; the first / last chunk of a row may be partial and falls back to scalar stores.
   __syncthreads();
+  if constexpr (kPalm) {   // palm = (v95 + v22) / 2 of the (centred) staged vertices, in place of the wrist
+    if (blockIdx.y == 0 && t < HG && s_side[t] >= 0) {
+      const int hand = g0 + t;
+      const float* sp = &s_stage[t][(int)(((size_t)hand * NV * 3) & 3)];
+      write_joint(p, hand, 0, (sp[3 * PALM_VA + 0] + sp[3 * PALM_VB + 0]) * 0.5f,
+                  (sp[3 * PALM_VA + 1] + sp[3 * PALM_VB + 1]) * 0.5f, (sp[3 * PALM_VA + 2] + sp[3 * PALM_VB + 2]) * 0.5f,
+                  s_pc[t]);
+    }
+  }
   {
     const int v0 = blockIdx.y * VPB;
     const int nfl = min(VPB, NV - v0) * 3;
@@ -415,7 +441,7 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
         if (full) {
           if (p.verts) *reinterpret_cast<float4*>(p.verts + gidx + i0) = q;
           if (p.verts_camed && p.cam) *reinterpret_cast<float4*>(p.verts_camed + gidx + i0) = make_float4(c4[0], c4[1], c4[2], c4[3]);
-          if (p.gather) {
+          if (kGather && p.gather) {
             const unsigned long long off = slot_off + (gg + i0) * 4;
             if (slot_mc) multimem_st_v4(reinterpret_cast<float*>(p.mc_base + off), q);
             else for (int r = 0; r < p.world; ++r) *reinterpret_cast<float4*>(p.peer_base[r] + off) = q;
@@ -427,7 +453,7 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
             if (i < 0 || i >= nfl) continue;
             if (p.verts) p.verts[gidx + i] = e[k];
             if (p.verts_camed && p.cam) p.verts_camed[gidx + i] = c4[k];
-            if (p.gather) {
+            if (kGather && p.gather) {
               const unsigned long long off = slot_off + (gg + i) * 4;
               if (slot_mc) multimem_st_f32(reinterpret_cast<float*>(p.mc_base + off), e[k]);
               else for (int r = 0; r < p.world; ++r) *reinterpret_cast<float*>(p.peer_base[r] + off) = e[k];
@@ -443,7 +469,7 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
   // Every CTA (also the ones beyond n) counts itself done after a system-scope fence; the last one to finish
   // publishes step+1 in the flag word flags[rank] of EVERY rank (release, system scope): whoever acquires that
   // value sees all vertices and counts of this launch.  No separate barrier kernel, no NCCL call.
-  if (p.gather) {
+  if (kGather && p.gather) {
     __syncthreads();
     if (t == 0) {
       __threadfence_system();
@@ -460,6 +486,12 @@ __global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) {
     }
   }
 }
+
+__global__ void __launch_bounds__(VPB) mano_forward_kernel(const ManoParams p) { mano_forward_body<POSE_AXISANG, false>(p); }
+
+// the other forms of acr_b200_mano_layer_forward (axis angle without the palm is mano_forward_kernel itself)
+template <int kPose, bool kPalm>
+__global__ void __launch_bounds__(VPB) mano_layer_forward_kernel(const ManoParams p) { mano_forward_body<kPose, kPalm>(p); }
 
 // stream-ordered wait until the stores of the most recent gather launch of EVERY rank have landed in this rank's memory
 __global__ void gather_wait_kernel(const unsigned long long* flags, const unsigned long long* step_dev, int world) {
@@ -548,7 +580,10 @@ struct ManoGradParams {
 
 constexpr size_t GRAD_DYN_SMEM = (size_t)(HG * DUVP_STRIDE + 3 * VPB * HG + 3 * NK * HG) * sizeof(float);
 
-__global__ void __launch_bounds__(VPB) mano_backward_vertex_kernel(const ManoGradParams p) {
+// kPose / kPalm as in mano_forward_body: with the palm, half of output joint 0's cotangent joins the du of each of
+// vertices 95 and 22.
+template <int kPose, bool kPalm>
+__device__ __forceinline__ void mano_backward_vertex_body(const ManoGradParams p) {
   __shared__ __align__(16) float s_pm[NK][HG];
   __shared__ __align__(16) float s_A[HG][16][12];
   __shared__ float s_R[HG][16][9];
@@ -565,7 +600,8 @@ __global__ void __launch_bounds__(VPB) mano_backward_vertex_kernel(const ManoGra
   const float* __restrict__ m = p.model;
   {
     const int h = t >> 4, j = t & 15;
-    rebuild_transforms<true>(g0 + h < p.n, m, p.poses, p.betas, g0 + h, h, j, p.center_src, s_pm, s_A, s_R, s_J, s_G, s_ctr);
+    rebuild_transforms<true, kPose>(g0 + h < p.n, m, p.poses, p.betas, g0 + h, h, j, p.center_src, s_pm, s_A, s_R, s_J,
+                                    s_G, s_ctr);
   }
   const int v0 = blockIdx.y * VPB;
   const int nv = min(VPB, NV - v0);
@@ -594,6 +630,10 @@ __global__ void __launch_bounds__(VPB) mano_backward_vertex_kernel(const ManoGra
         if (tip >= 0 && p.djoints) {
           const float* d = p.djoints + ((size_t)hand * 21 + c_joint_inv[16 + tip]) * 3;
           du[0] += d[0]; du[1] += d[1]; du[2] += d[2];
+        }
+        if (kPalm && (v == PALM_VA || v == PALM_VB) && p.djoints) {
+          const float* d = p.djoints + (size_t)hand * 21 * 3;
+          du[0] += 0.5f * d[0]; du[1] += 0.5f * d[1]; du[2] += 0.5f * d[2];
         }
       }
       float T[12];
@@ -677,7 +717,11 @@ __global__ void __launch_bounds__(VPB) mano_backward_vertex_kernel(const ManoGra
   }
 }
 
-__global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGradParams p) {
+// kPose / kPalm as in mano_forward_body.  With the palm, the kinematic joint 0 is no output: its cotangent reached
+// the two palm vertices in the vertex kernel, so it is neither the wrist's dt nor part of the centre term here.
+// With POSE_ROTMAT, the rotation cotangent goes through the SO(3) projection's VJP into dposes (n,16,3,3).
+template <int kPose, bool kPalm>
+__device__ __forceinline__ void mano_backward_chain_body(const ManoGradParams p) {
   __shared__ __align__(16) float s_pm[NK][HG];
   __shared__ __align__(16) float s_A[HG][16][12];
   __shared__ float s_R[HG][16][9];
@@ -693,7 +737,8 @@ __global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGrad
   const int t = threadIdx.x, h = t >> 4, j = t & 15;
   const int hand = blockIdx.x * HG + h;
   const bool valid = hand < p.n;
-  rebuild_transforms<true>(valid, p.model, p.poses, p.betas, hand, h, j, p.center_src, s_pm, s_A, s_R, s_J, s_G, s_ctr);
+  rebuild_transforms<true, kPose>(valid, p.model, p.poses, p.betas, hand, h, j, p.center_src, s_pm, s_A, s_R, s_J, s_G,
+                                  s_ctr);
   const float* __restrict__ m = p.model;
   // ---- partials of the vertex kernel, summed over the chunks in order
   float dA[12], dpm[9], dpb = 0.f;
@@ -721,7 +766,7 @@ __global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGrad
       if (p.have_partials)   // sum of du = dverts + fingertip joint cotangents
         for (int ch = 0; ch < NCHUNK; ++ch) d -= p.ws[((size_t)hand * NCHUNK + ch) * WS_STRIDE + WS_DU + j];
       if (p.djoints)
-        for (int s = 0; s < 16; ++s) d -= p.djoints[((size_t)hand * 21 + c_joint_inv[s]) * 3 + j];
+        for (int s = kPalm ? 1 : 0; s < 16; ++s) d -= p.djoints[((size_t)hand * 21 + c_joint_inv[s]) * 3 + j];
     }
     s_dctr[h][j] = d;
   }
@@ -730,7 +775,7 @@ __global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGrad
   {
     const float* G = s_G[h][j];
     float dt[3] = {0.f, 0.f, 0.f};
-    if (valid && p.djoints) {
+    if (valid && p.djoints && !(kPalm && j == 0)) {
       const float* d = p.djoints + ((size_t)hand * 21 + c_joint_inv[j]) * 3;
       dt[0] = d[0]; dt[1] = d[1]; dt[2] = d[2];
     }
@@ -816,16 +861,24 @@ __global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGrad
   }
   __syncthreads();
   if (!valid) return;
-  // ---- Rodrigues backward (pose map = R - I for joints 1..15)
+  // ---- Rodrigues / SO(3) projection backward (pose map = R - I for joints 1..15)
   if (p.dposes) {
     float g[9];
 #pragma unroll
     for (int e = 0; e < 9; ++e) g[e] = s_dR[h][j][e] + dpm[e];
-    const float* ps = p.poses + (size_t)hand * 48 + j * 3;
-    float da[3];
-    rodrigues_vjp(ps[0] + m[OFF_HM + j * 3 + 0], ps[1] + m[OFF_HM + j * 3 + 1], ps[2] + m[OFF_HM + j * 3 + 2], g, da);
-    float* o = p.dposes + (size_t)hand * 48 + j * 3;
-    o[0] = da[0]; o[1] = da[1]; o[2] = da[2];
+    if constexpr (kPose == POSE_ROTMAT) {
+      const size_t off = ((size_t)hand * 16 + j) * 9;
+      float dM[9];
+      so3_project_vjp(p.poses + off, g, dM);
+#pragma unroll
+      for (int e = 0; e < 9; ++e) p.dposes[off + e] = dM[e];
+    } else {
+      const float* ps = p.poses + (size_t)hand * 48 + j * 3;
+      float da[3];
+      rodrigues_vjp(ps[0] + m[OFF_HM + j * 3 + 0], ps[1] + m[OFF_HM + j * 3 + 1], ps[2] + m[OFF_HM + j * 3 + 2], g, da);
+      float* o = p.dposes + (size_t)hand * 48 + j * 3;
+      o[0] = da[0]; o[1] = da[1]; o[2] = da[2];
+    }
   }
   // ---- betas: the shape rows of the vertices plus J = JT + JS . beta
   if (p.dbetas && j < 10) {
@@ -835,6 +888,23 @@ __global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGrad
       for (int c = 0; c < 3; ++c) d = fmaf(m[OFF_JS + (s * 3 + c) * 10 + j], s_dJ[h][s][c], d);
     p.dbetas[(size_t)hand * 10 + j] = d;
   }
+}
+
+__global__ void __launch_bounds__(VPB) mano_backward_vertex_kernel(const ManoGradParams p) {
+  mano_backward_vertex_body<POSE_AXISANG, false>(p);
+}
+__global__ void __launch_bounds__(VPB) mano_backward_chain_kernel(const ManoGradParams p) {
+  mano_backward_chain_body<POSE_AXISANG, false>(p);
+}
+
+// the other forms of acr_b200_mano_layer_backward
+template <int kPose, bool kPalm>
+__global__ void __launch_bounds__(VPB) mano_layer_backward_vertex_kernel(const ManoGradParams p) {
+  mano_backward_vertex_body<kPose, kPalm>(p);
+}
+template <int kPose, bool kPalm>
+__global__ void __launch_bounds__(VPB) mano_layer_backward_chain_kernel(const ManoGradParams p) {
+  mano_backward_chain_body<kPose, kPalm>(p);
 }
 
 }  // namespace acr
@@ -993,6 +1063,91 @@ extern "C" int acr_b200_mano_backward(const float* model, int side, const float*
   mano_backward_chain_kernel<<<ceil_div(n, HG), VPB, 0, s>>>(p);
   ACR_CHECK_LAUNCH();
   return ACR_B200_OK;
+}
+
+// ------------------------------------------------------------------------------------- ManoLayer entry points
+// Argument checks shared by acr_b200_mano_layer_forward / _backward -> the centre's source joint (-1 none).
+static int layer_args(const char* what, int side, int pose_mode, int center_idx, int root_palm, int* center_src) {
+  ACR_CHECK_ARG(side == 0 || side == 1, "%s: side must be 0 (left) or 1 (right)", what);
+  ACR_CHECK_ARG(pose_mode == ACR_B200_POSE_AXISANG || pose_mode == ACR_B200_POSE_ROTMAT, "%s: unknown pose_mode %d", what,
+                pose_mode);
+  ACR_CHECK_ARG(center_idx >= -1 && center_idx < 21, "%s: center_idx out of range", what);
+  static const int perm[21] = {0, 13, 14, 15, 16, 1, 2, 3, 17, 4, 5, 6, 18, 10, 11, 12, 19, 7, 8, 9, 20};
+  *center_src = center_idx >= 0 ? perm[center_idx] : -1;
+  if (*center_src >= 16) {
+    set_error("%s: centring on a fingertip joint (center_idx=%d) is not supported", what, center_idx);
+    return ACR_B200_ENOTSUP;
+  }
+  if (root_palm && center_idx == 0) {
+    set_error("%s: centring on the palm (center_idx=0 with root_palm) is not supported", what);
+    return ACR_B200_ENOTSUP;
+  }
+  return ACR_B200_OK;
+}
+
+extern "C" int acr_b200_mano_layer_forward(const float* model, int side, const float* pose, int pose_mode,
+                                           const float* betas, int n, int center_idx, int root_palm, float* verts,
+                                           float* joints, float* center, void* stream) {
+  ACR_CHECK_ARG(n >= 0, "mano_layer_forward: n < 0");
+  if (n == 0) return ACR_B200_OK;
+  ACR_CHECK_ARG(model && pose && betas, "mano_layer_forward: model / pose / betas are null");
+  ACR_CHECK_ARG((uintptr_t)verts % 16 == 0, "mano_layer_forward: verts must be 16-byte aligned");
+  int center_src;
+  if (const int rc = layer_args("mano_layer_forward", side, pose_mode, center_idx, root_palm, &center_src)) return rc;
+  ManoParams p = {};
+  p.model[0] = p.model[1] = model;
+  p.poses = pose; p.betas = betas; p.default_side = side; p.n_max = n; p.center_src = center_src;
+  p.verts = verts; p.joints = joints; p.center = center;
+  const dim3 grid(ceil_div(n, HG), ceil_div(NV, VPB));
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (pose_mode == ACR_B200_POSE_ROTMAT) {
+    if (root_palm) mano_layer_forward_kernel<POSE_ROTMAT, true><<<grid, VPB, 0, s>>>(p);
+    else mano_layer_forward_kernel<POSE_ROTMAT, false><<<grid, VPB, 0, s>>>(p);
+  } else {
+    if (root_palm) mano_layer_forward_kernel<POSE_AXISANG, true><<<grid, VPB, 0, s>>>(p);
+    else mano_forward_kernel<<<grid, VPB, 0, s>>>(p);
+  }
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}
+
+template <int kPose, bool kPalm>
+static int launch_layer_backward(const ManoGradParams& p, bool partials, cudaStream_t s) {
+  if (partials) {
+    static unsigned long long smem_done = 0;
+    ACR_CHECK_CUDA(ensure_dynamic_smem(mano_layer_backward_vertex_kernel<kPose, kPalm>, (int)GRAD_DYN_SMEM, &smem_done));
+    mano_layer_backward_vertex_kernel<kPose, kPalm><<<dim3(ceil_div(p.n, HG), NCHUNK), VPB, GRAD_DYN_SMEM, s>>>(p);
+    ACR_CHECK_LAUNCH();
+  }
+  mano_layer_backward_chain_kernel<kPose, kPalm><<<ceil_div(p.n, HG), VPB, 0, s>>>(p);
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}
+
+extern "C" int acr_b200_mano_layer_backward(const float* model, int side, const float* pose, int pose_mode,
+                                            const float* betas, int n, int center_idx, int root_palm,
+                                            const float* dverts, const float* djoints, const float* dcenter,
+                                            float* workspace, float* dpose, float* dbetas, void* stream) {
+  ACR_CHECK_ARG(n >= 0, "mano_layer_backward: n < 0");
+  if (n == 0) return ACR_B200_OK;
+  ACR_CHECK_ARG(model && pose && betas, "mano_layer_backward: model / pose / betas are null");
+  int center_src;
+  if (const int rc = layer_args("mano_layer_backward", side, pose_mode, center_idx, root_palm, &center_src)) return rc;
+  const bool partials = dverts || djoints;
+  ACR_CHECK_ARG(!partials || workspace, "mano_layer_backward: workspace is null (acr_b200_mano_backward_workspace_floats)");
+  if (!dpose && !dbetas) return ACR_B200_OK;
+  if (pose_mode == ACR_B200_POSE_AXISANG && !root_palm)
+    return acr_b200_mano_backward(model, side, pose, betas, n, center_idx, dverts, djoints, dcenter, workspace, dpose,
+                                  dbetas, stream);
+  ManoGradParams p = {};
+  p.model = model; p.side = side; p.poses = pose; p.betas = betas; p.n = n; p.center_src = center_src;
+  p.dverts = dverts; p.djoints = djoints; p.dcenter = dcenter; p.ws = workspace; p.have_partials = partials;
+  p.dposes = dpose; p.dbetas = dbetas;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (pose_mode == ACR_B200_POSE_ROTMAT)
+    return root_palm ? launch_layer_backward<POSE_ROTMAT, true>(p, partials, s)
+                     : launch_layer_backward<POSE_ROTMAT, false>(p, partials, s);
+  return launch_layer_backward<POSE_AXISANG, true>(p, partials, s);
 }
 
 extern "C" int acr_b200_gather_wait(const acr_b200_gather* g, void* stream) {

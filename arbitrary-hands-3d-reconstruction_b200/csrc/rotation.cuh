@@ -72,6 +72,141 @@ __device__ __forceinline__ void rodrigues_vjp(float ax, float ay, float az, cons
   da[2] = sa * dq[3] + dang * (bz / ang);
 }
 
+// ------------------------------------------------------------------------------ SO(3) projection (batch_rotprojs)
+// The reference (mano/manolayer.py:436-453) takes the SVD M = U S V^T of every input matrix, forms the orthogonal
+// polar factor Q = U V^T and negates column 2 of Q when det Q < 0.  Here, per thread and in fp64: a fixed-sweep
+// cyclic Jacobi eigensolve of A = M^T M gives V (a proper rotation) and S^2; then u_i = M v_i normalised for the two
+// largest singular values (Gram-Schmidt on the second), u_3 = sign(det M) (u_1 x u_2), and Q = sum_i u_i v_i^T.
+// Contract: M of rank >= 2 gives a finite orthogonal Q (at rank 2, det M is zero up to rounding and its computed
+// sign picks the orientation).  Rank <= 1 is outside it -- the reference's own result is arbitrary there -- and
+// gives NaN.  All indexing is compile-time, so nothing lives in local memory.
+template <int p, int q>
+__device__ __forceinline__ void jacobi_rotate(double (&a)[3][3], double (&v)[3][3]) {
+  constexpr int r = 3 - p - q;
+  const double apq = a[p][q];
+  if (apq == 0.0) return;
+  const double th = (a[q][q] - a[p][p]) / (2.0 * apq);
+  const double t = copysign(1.0, th) / (fabs(th) + sqrt(fma(th, th, 1.0)));   // th = +-inf -> t = 0
+  const double c = rsqrt(fma(t, t, 1.0)), s = t * c;
+  const double app = a[p][p] - t * apq, aqq = a[q][q] + t * apq;
+  const double arp = c * a[r][p] - s * a[r][q], arq = s * a[r][p] + c * a[r][q];
+  a[p][p] = app; a[q][q] = aqq; a[p][q] = a[q][p] = 0.0;
+  a[r][p] = a[p][r] = arp; a[r][q] = a[q][r] = arq;
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double vp = v[i][p], vq = v[i][q];
+    v[i][p] = c * vp - s * vq; v[i][q] = s * vp + c * vq;
+  }
+}
+
+// swap eigenpairs i < k so that lam[i] >= lam[k]; negating one column keeps det V = +1
+template <int i, int k>
+__device__ __forceinline__ void eig_order(double (&lam)[3], double (&v)[3][3]) {
+  if (lam[i] >= lam[k]) return;
+  const double l = lam[i]; lam[i] = lam[k]; lam[k] = l;
+#pragma unroll
+  for (int e = 0; e < 3; ++e) { const double x = v[e][i]; v[e][i] = v[e][k]; v[e][k] = -x; }
+}
+
+// M (row-major 3x3, fp32) -> its orthogonal polar factor Q (fp64, row-major) and whether det Q < 0 (`flip`; the
+// reference then negates column 2 of Q).  The output rotation is Q diag(1, 1, flip ? -1 : 1).
+__device__ __forceinline__ void polar_factor(const float* __restrict__ Mf, double (&Q)[3][3], bool& flip) {
+  double M[3][3], a[3][3], v[3][3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) { M[r][c] = (double)Mf[r * 3 + c]; v[r][c] = r == c ? 1.0 : 0.0; }
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) a[r][c] = M[0][r] * M[0][c] + M[1][r] * M[1][c] + M[2][r] * M[2][c];
+  // quadratic convergence: 6 cyclic sweeps take any 3x3 well below fp64 rounding
+#pragma unroll 1
+  for (int sweep = 0; sweep < 6; ++sweep) {
+    jacobi_rotate<0, 1>(a, v);
+    jacobi_rotate<0, 2>(a, v);
+    jacobi_rotate<1, 2>(a, v);
+  }
+  double lam[3] = {a[0][0], a[1][1], a[2][2]};
+  eig_order<0, 1>(lam, v);
+  eig_order<1, 2>(lam, v);
+  eig_order<0, 1>(lam, v);
+  double u[2][3];
+#pragma unroll
+  for (int k = 0; k < 2; ++k)
+#pragma unroll
+    for (int r = 0; r < 3; ++r) u[k][r] = M[r][0] * v[0][k] + M[r][1] * v[1][k] + M[r][2] * v[2][k];
+  double n0 = rsqrt(u[0][0] * u[0][0] + u[0][1] * u[0][1] + u[0][2] * u[0][2]);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) u[0][r] *= n0;
+  const double d01 = u[0][0] * u[1][0] + u[0][1] * u[1][1] + u[0][2] * u[1][2];
+#pragma unroll
+  for (int r = 0; r < 3; ++r) u[1][r] -= d01 * u[0][r];
+  double n1 = rsqrt(u[1][0] * u[1][0] + u[1][1] * u[1][1] + u[1][2] * u[1][2]);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) u[1][r] *= n1;
+  const double detM = M[0][0] * (M[1][1] * M[2][2] - M[1][2] * M[2][1]) - M[0][1] * (M[1][0] * M[2][2] - M[1][2] * M[2][0]) +
+                      M[0][2] * (M[1][0] * M[2][1] - M[1][1] * M[2][0]);
+  flip = detM < 0.0;
+  const double sg = flip ? -1.0 : 1.0;
+  const double u2[3] = {sg * (u[0][1] * u[1][2] - u[0][2] * u[1][1]), sg * (u[0][2] * u[1][0] - u[0][0] * u[1][2]),
+                        sg * (u[0][0] * u[1][1] - u[0][1] * u[1][0])};
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) Q[r][c] = u[0][r] * v[c][0] + u[1][r] * v[c][1] + u2[r] * v[c][2];
+}
+
+// batch_rotprojs of one matrix: M (row-major, fp32) -> R = Q D (row-major, fp32)
+__device__ __forceinline__ void so3_project(const float* __restrict__ M, float* __restrict__ R) {
+  double Q[3][3];
+  bool flip;
+  polar_factor(M, Q, flip);
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    R[r * 3 + 0] = (float)Q[r][0]; R[r * 3 + 1] = (float)Q[r][1];
+    R[r * 3 + 2] = (float)(flip ? -Q[r][2] : Q[r][2]);
+  }
+}
+
+// Vector-Jacobian product of so3_project(): g (cotangent of R, row-major) -> dM.  With P = Q^T M (symmetric),
+// B = Q^T (g D) and k = axial(B - B^T):  z = ((tr P) I - P)^-1 k,  dM = Q [z]x.  (tr P) I - P has the eigenvalues
+// s_j + s_k, so this is finite whenever no two singular values sum to zero -- in particular at exact rotations,
+// where the SVD's own derivative (1 / (s_i^2 - s_j^2)) is not.
+__device__ __forceinline__ void so3_project_vjp(const float* __restrict__ Mf, const float* __restrict__ g,
+                                                float* __restrict__ dM) {
+  double Q[3][3];
+  bool flip;
+  polar_factor(Mf, Q, flip);
+  double P[3][3], B[3][3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const double gd = c == 2 && flip ? -1.0 : 1.0;
+      P[r][c] = Q[0][r] * (double)Mf[0 * 3 + c] + Q[1][r] * (double)Mf[1 * 3 + c] + Q[2][r] * (double)Mf[2 * 3 + c];
+      B[r][c] = gd * (Q[0][r] * (double)g[0 * 3 + c] + Q[1][r] * (double)g[1 * 3 + c] + Q[2][r] * (double)g[2 * 3 + c]);
+    }
+  const double k0 = B[2][1] - B[1][2], k1 = B[0][2] - B[2][0], k2 = B[1][0] - B[0][1];
+  const double tr = P[0][0] + P[1][1] + P[2][2];
+  // A = tr I - P (symmetrised), solved through its adjugate
+  const double a00 = tr - P[0][0], a11 = tr - P[1][1], a22 = tr - P[2][2];
+  const double a01 = -0.5 * (P[0][1] + P[1][0]), a02 = -0.5 * (P[0][2] + P[2][0]), a12 = -0.5 * (P[1][2] + P[2][1]);
+  const double c00 = a11 * a22 - a12 * a12, c01 = a02 * a12 - a01 * a22, c02 = a01 * a12 - a02 * a11;
+  const double c11 = a00 * a22 - a02 * a02, c12 = a01 * a02 - a00 * a12, c22 = a00 * a11 - a01 * a01;
+  const double inv = 1.0 / (a00 * c00 + a01 * c01 + a02 * c02);
+  const double z0 = (c00 * k0 + c01 * k1 + c02 * k2) * inv;
+  const double z1 = (c01 * k0 + c11 * k1 + c12 * k2) * inv;
+  const double z2 = (c02 * k0 + c12 * k1 + c22 * k2) * inv;
+  // [z]x = [[0, -z2, z1], [z2, 0, -z0], [-z1, z0, 0]]
+#pragma unroll
+  for (int r = 0; r < 3; ++r) {
+    dM[r * 3 + 0] = (float)(Q[r][1] * z2 - Q[r][2] * z1);
+    dM[r * 3 + 1] = (float)(Q[r][2] * z0 - Q[r][0] * z2);
+    dM[r * 3 + 2] = (float)(Q[r][0] * z1 - Q[r][1] * z0);
+  }
+}
+
 // rotation_matrix_to_angle_axis (acr/utils.py:334-360) of a row-major 3x3 (not necessarily orthonormal)
 // matrix: 4-case quaternion on the TRANSPOSED matrix (:862-906), atan2 form (:803-823), NaN -> 0.
 __device__ __forceinline__ void rotmat_to_aa(const float* __restrict__ R, float* __restrict__ aa) {

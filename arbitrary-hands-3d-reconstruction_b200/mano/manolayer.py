@@ -7,6 +7,10 @@ the reference forward (:104-276) become a single ``acr_b200_mano_forward`` call.
 The layer is differentiable with respect to the pose (or PCA coefficients), betas and ``th_trans``: with grad
 enabled and pose or betas requiring grad, the kernel runs inside ``_ManoFunction``, whose backward is the fused
 ``acr_b200_mano_backward``.  Otherwise the forward makes exactly the launch it makes without autograd.
+
+Rotation-matrix joints (``use_pca=False, joint_rot_mode='rotmat'``, reference :151-162) and ``root_palm``
+(:248-250) run through ``acr_b200_mano_layer_forward`` / ``_backward`` instead (``_ManoLayerFunction``): the
+SO(3) projection of every input matrix and its gradient are fused into the same kernels.
 """
 from __future__ import annotations
 
@@ -17,6 +21,7 @@ import torch
 from torch.autograd.function import once_differentiable
 from torch.nn import Module
 
+from acr_b200 import lib as _lib
 from acr_b200 import ops as _ops
 from mano.assets import get_asset
 
@@ -50,18 +55,59 @@ class _ManoFunction(torch.autograd.Function):
         return dpose, dbetas, None, None, None
 
 
+class _ManoLayerFunction(torch.autograd.Function):
+    """(pose: (n,16,3,3) matrices or (n,48) axis angles without the mean pose, betas (n,10)) -> (verts, joints,
+    center) of one side, with ``root_palm``; the backward is the fused kernel pair (first order only)."""
+
+    @staticmethod
+    def forward(ctx, pose, betas, model, side, pose_mode, center_idx, root_palm):
+        out = _ops.mano_layer_forward(model, side, pose, pose_mode, betas, center_idx, root_palm)
+        ctx.save_for_backward(pose, betas)
+        ctx.args = (model, side, pose_mode, center_idx, root_palm)
+        ctx.set_materialize_grads(False)     # an unused output's cotangent stays None and reaches the kernel as NULL
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dverts, djoints, dcenter):
+        pose, betas = ctx.saved_tensors
+        model, side, pose_mode, center_idx, root_palm = ctx.args
+        if center_idx is None:
+            dcenter = None                   # the centre output is zero and does not depend on the inputs
+        none = (None,) * 7
+        if dverts is None and djoints is None and dcenter is None:
+            return none
+        dpose, dbetas = _ops.mano_layer_backward(model, side, pose, pose_mode, betas, center_idx, root_palm, dverts,
+                                                 djoints, dcenter, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        return (dpose, dbetas) + none[2:]
+
+
+def _rodrigues(aa: torch.Tensor) -> torch.Tensor:
+    """(M,3) axis angles -> (M,3,3), the reference's half-angle quaternion form (its batch_rodrigues); used once, for
+    the ``th_hands_mean_rotmat`` buffer."""
+    ang = torch.norm(aa + 1e-8, dim=1, keepdim=True)
+    q = torch.cat([torch.cos(ang * 0.5), torch.sin(ang * 0.5) * (aa / ang)], 1)
+    w, x, y, z = (q / q.norm(dim=1, keepdim=True)).unbind(1)
+    return torch.stack([w * w + x * x - y * y - z * z, 2 * x * y - 2 * w * z, 2 * w * y + 2 * x * z,
+                        2 * w * z + 2 * x * y, w * w - x * x + y * y - z * z, 2 * y * z - 2 * w * x,
+                        2 * x * z - 2 * w * y, 2 * w * x + 2 * y * z, w * w - x * x - y * y + z * z], 1).view(-1, 3, 3)
+
+
 class ManoLayer(Module):
     __constants__ = ['use_pca', 'rot', 'ncomps', 'kintree_parents', 'side', 'center_idx', 'joint_rot_mode']
 
     def __init__(self, center_idx=None, flat_hand_mean=True, ncomps=6, side='right', mano_root='model_data/mano/',
                  use_pca=True, root_rot_mode='axisang', joint_rot_mode='axisang', robust_rot=False, asset=None):
         super().__init__()
-        if root_rot_mode != 'axisang' or joint_rot_mode != 'axisang':
+        # as in the reference, any joint_rot_mode but 'axisang' without PCA takes (n,16,3,3) matrices, and that
+        # branch ignores root_rot_mode
+        self.rotmat = not use_pca and joint_rot_mode != 'axisang'
+        if not self.rotmat and root_rot_mode != 'axisang':
             # the reference's 6D-root branch references an undefined name (manolayer.py:148-150)
-            raise NotImplementedError("only root_rot_mode='axisang', joint_rot_mode='axisang' are supported")
+            raise NotImplementedError("only root_rot_mode='axisang' is supported with axis-angle joints")
         self.center_idx = center_idx
         self.robust_rot = robust_rot
-        self.rot = 3
+        self.rot = 3 if root_rot_mode == 'axisang' else 6
         self.flat_hand_mean = flat_hand_mean
         self.side = side
         self.use_pca = use_pca
@@ -81,9 +127,13 @@ class ManoLayer(Module):
         self.register_buffer('th_faces', T(np.asarray(smpl_data['f']).astype(np.int32), np.int32).long())
         hands_mean = np.zeros(hands_components.shape[1], np.float32) if flat_hand_mean \
             else np.asarray(smpl_data['hands_mean'], np.float32).copy()
-        self.register_buffer('th_hands_mean', T(hands_mean).unsqueeze(0))
-        self.register_buffer('th_comps', T(hands_components))
-        self.register_buffer('th_selected_comps', T(hands_components[:ncomps]))
+        if self.rotmat:
+            # the reference keeps the mean pose as matrices and never applies it in forward
+            self.register_buffer('th_hands_mean_rotmat', _rodrigues(T(hands_mean).view(15, 3)).reshape(15, 3, 3))
+        else:
+            self.register_buffer('th_hands_mean', T(hands_mean).unsqueeze(0))
+            self.register_buffer('th_comps', T(hands_components))
+            self.register_buffer('th_selected_comps', T(hands_components[:ncomps]))
         self.kintree_table = smpl_data['kintree_table']
         self.kintree_parents = list(np.asarray(self.kintree_table)[0].tolist())
         self._packed = None
@@ -91,8 +141,10 @@ class ManoLayer(Module):
 
     # packed constants follow the *current* buffers (MANOWrapper flips th_shapedirs in place)
     def packed_model(self) -> torch.Tensor:
-        bufs = (self.th_shapedirs, self.th_posedirs, self.th_v_template, self.th_J_regressor, self.th_weights,
-                self.th_hands_mean)
+        # rotation-matrix layers have no axis-angle mean pose: the packed one is zero and unused
+        hm = None if self.rotmat else self.th_hands_mean
+        bufs = (self.th_shapedirs, self.th_posedirs, self.th_v_template, self.th_J_regressor, self.th_weights) + \
+            (() if hm is None else (hm,))
         key = tuple((b._version, b.data_ptr(), str(b.device)) for b in bufs)
         if self._packed is None or key != self._packed_key:
             asset = dict(shapedirs=self.th_shapedirs.detach().cpu().numpy(),
@@ -100,18 +152,24 @@ class ManoLayer(Module):
                          v_template=self.th_v_template[0].detach().cpu().numpy(),
                          J_regressor=self.th_J_regressor.detach().cpu().numpy(),
                          weights=self.th_weights.detach().cpu().numpy(),
-                         hands_mean=self.th_hands_mean[0].detach().cpu().numpy())
+                         hands_mean=np.zeros(45, np.float32) if hm is None else hm[0].detach().cpu().numpy())
             self._packed = _ops.pack_mano_model(asset, False, self.th_shapedirs.device)
             self._packed_key = key
         return self._packed
 
     def forward(self, th_pose_coeffs, th_betas=_ZERO1, th_trans=_ZERO1, root_palm=torch.Tensor([0]),
                 share_betas=torch.Tensor([0])):
-        if bool(root_palm):
-            raise NotImplementedError("root_palm=True is not on the ACR hot path")
+        palm = bool(root_palm)
         batch_size = th_pose_coeffs.shape[0]
         pose = th_pose_coeffs
-        if self.use_pca:
+        if self.rotmat:
+            assert pose.dim() == 4, ('When not self.use_pca, th_pose_coeffs should have 4 dims, got {}'.format(
+                pose.dim()))
+            assert pose.shape[2:4] == (3, 3), ('When not self.use_pca, th_pose_coeffs have 3x3 matrix for two '
+                                               'last dims, got {}'.format(pose.shape[2:4]))
+            if pose.shape[1] != 16:
+                raise ValueError(f"rotation-matrix pose must be (n,16,3,3), got {tuple(pose.shape)}")
+        elif self.use_pca:
             pose = torch.cat([pose[:, :3], pose[:, 3:3 + self.ncomps].mm(self.th_selected_comps)], 1)
         if th_betas is None or th_betas.numel() == 1:
             betas = self.th_betas.expand(batch_size, 10)
@@ -121,9 +179,18 @@ class ManoLayer(Module):
                 betas = betas.mean(0, keepdim=True).expand(betas.shape[0], 10)
         use_trans = not (th_trans is None or th_trans is _ZERO1 or bool(torch.norm(th_trans) == 0))
         center_idx = None if use_trans else self.center_idx
+        if palm and center_idx == 0:
+            raise NotImplementedError("centring on the palm (center_idx=0 with root_palm) is not supported")
         side = 1 if self.side == 'right' else 0
         model = self.packed_model()
-        if torch.is_grad_enabled() and (pose.requires_grad or betas.requires_grad):
+        if self.rotmat or palm:
+            mode = _lib.POSE_ROTMAT if self.rotmat else _lib.POSE_AXISANG
+            p = pose if self.rotmat else pose[:, :48]
+            if torch.is_grad_enabled() and (p.requires_grad or betas.requires_grad):
+                verts, jtr, center = _ManoLayerFunction.apply(p, betas, model, side, mode, center_idx, palm)
+            else:
+                verts, jtr, center = _ops.mano_layer_forward(model, side, p, mode, betas, center_idx, palm)
+        elif torch.is_grad_enabled() and (pose.requires_grad or betas.requires_grad):
             verts, jtr, center = _ManoFunction.apply(pose[:, :48], betas, model, side, center_idx)
         else:
             out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose[:, :48],

@@ -124,6 +124,32 @@ int acr_b200_mano_backward(const float* model, int side, const float* poses, con
                            int center_idx, const float* dverts, const float* djoints, const float* dcenter,
                            float* workspace, float* dposes, float* dbetas, void* stream);
 
+/* ManoLayer.forward of one side with every pose input and root_palm (mano/manolayer.py:104-276), and its backward.
+ *   pose_mode ACR_B200_POSE_AXISANG : pose (n,48) axis angles WITHOUT the mean pose, as acr_b200_mano_forward.
+ *   pose_mode ACR_B200_POSE_ROTMAT  : pose (n,16,3,3) row-major matrices, unprojected (use_pca=False,
+ *             joint_rot_mode='rotmat', :151-162).  Each is projected like batch_rotprojs (:436-453): Q = U V^T of
+ *             its SVD M = U S V^T, column 2 negated when det Q < 0.  No mean pose is applied, as in the reference.
+ *             Any matrix of rank >= 2 gives a finite orthogonal result; rank <= 1 is outside the contract (the
+ *             reference's own result is arbitrary there) and gives NaN.  The gradient dpose (n,16,3,3) is the
+ *             polar factor's: finite at exact rotations (where the SVD's derivative is not) and whenever no two
+ *             singular values sum to zero.
+ *   root_palm : nonzero => output joint 0 is the palm, (v95 + v22) / 2, instead of the wrist (:248-250).
+ *   center_idx : as in acr_b200_mano_forward.  A fingertip, or the palm (0 with root_palm), is ACR_B200_ENOTSUP.
+ *   betas (n,10).  Outputs verts (n,778,3) (16-byte aligned), joints (n,21,3), center (n,3); any may be NULL.
+ * The backward takes the forward's arguments and the cotangents, and writes dpose (shaped like pose) and dbetas;
+ * cotangents, workspace and outputs as in acr_b200_mano_backward.  A bad side, pose_mode or centre is
+ * ACR_B200_EINVAL.  Axis angles without the palm make exactly the launches of acr_b200_mano_forward /
+ * acr_b200_mano_backward.                                                                                     */
+#define ACR_B200_POSE_AXISANG 0
+#define ACR_B200_POSE_ROTMAT 1
+int acr_b200_mano_layer_forward(const float* model, int side, const float* pose, int pose_mode, const float* betas,
+                                int n, int center_idx, int root_palm, float* verts, float* joints, float* center,
+                                void* stream);
+int acr_b200_mano_layer_backward(const float* model, int side, const float* pose, int pose_mode,
+                                 const float* betas, int n, int center_idx, int root_palm, const float* dverts,
+                                 const float* djoints, const float* dcenter, float* workspace, float* dpose,
+                                 float* dbetas, void* stream);
+
 /* Camera translation of every hand from its 21 joints: the closed-form weighted least squares of
  * estimate_translation_np (acr/utils.py:430-472) -- the reference's own fall-back for the host-side
  * cv2.solvePnPRansac loop (estimate_translation :474-519, called from vertices_kp3d_projection :403-407,
