@@ -36,7 +36,8 @@ _DEFAULTS = dict(
     temporal_optimization=False, smooth_coeff=4.0,         # config.py:29-30
     model_path=os.path.join(project_dir, "checkpoints", "wild.pkl"),
     mano_root=os.path.join(project_dir, "mano"),           # acr/mano_wrapper.py:22 uses 'mano/'
-    cam_trans_mode="lstsq",                                # 'lstsq' (device least squares, SURVEY 8f-1) | 'none'
+    cam_trans_mode="lstsq",                                # 'lstsq' (device least squares, SURVEY 8f-1) | 'pnp' (device
+                                                          # RANSAC-EPnP, the reference's cv2.solvePnPRansac) | 'none'
     return_maps=True,                                      # materialise NCHW fp32 maps lazily on access
     demo_mode="image", inputs=None, output_dir=None, save_dict_results=False,
 )

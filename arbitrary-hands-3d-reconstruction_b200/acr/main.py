@@ -71,9 +71,9 @@ class ACR(nn.Module):
         ml, mr = self.mano_regression.models()
         mano = _ops.mano_forward(ml, mr, bufs.poses, bufs.betas, bufs.hand_type, 1, self.mano_regression.center_idx,
                                  bufs.cam, bufs.offsets_out, n_dev=bufs.counts[2:3], peers=peers, counts=bufs.counts)
-        if args().cam_trans_mode == 'lstsq':
-            mano['cam_trans'] = _ops.cam_trans(mano['joints'], mano['pj2d'], args().focal_length, 512.0,
-                                               n_dev=bufs.counts[2:3])
+        if args().cam_trans_mode in ('lstsq', 'pnp'):
+            mano['cam_trans'] = _ops.cam_trans_mode(args().cam_trans_mode, mano['joints'], mano['pj2d'],
+                                                    args().focal_length, 512.0, n_dev=bufs.counts[2:3])
         return bufs, mano
 
     @torch.no_grad()

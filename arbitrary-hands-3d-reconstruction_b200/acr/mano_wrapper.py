@@ -40,10 +40,9 @@ class MANOWrapper(nn.Module):
         if 'pj2d_org' in out:
             outputs['pj2d_org'] = out['pj2d_org']
         # cam_trans: the reference runs cv2.solvePnPRansac per hand on the host (acr/utils.py:403-407,
-        # 414-519) only to feed the renderer.  'lstsq' = its own closed-form fall-back (estimate_translation_np
-        # :430-472) evaluated on the device, no D2H/H2D round trip (SURVEY.md 8f-1); 'none' skips it.
-        if args().cam_trans_mode == 'lstsq':
-            outputs['cam_trans'] = _ops.cam_trans(out['joints'], out['pj2d'], args().focal_length, 512.0)
-        else:
-            outputs['cam_trans'] = None
+        # 414-519) only to feed the renderer.  'pnp' = that RANSAC-EPnP on the device; 'lstsq' = its own
+        # closed-form fall-back (estimate_translation_np :430-472) on the device; neither makes a D2H/H2D round
+        # trip (SURVEY.md 8f-1); 'none' skips it.
+        outputs['cam_trans'] = _ops.cam_trans_mode(args().cam_trans_mode, out['joints'], out['pj2d'],
+                                                   args().focal_length, 512.0)
         return outputs

@@ -156,6 +156,34 @@ def cam_trans(j3d: torch.Tensor, pj2d: torch.Tensor, focal_length: float = 1265.
     return out
 
 
+def cam_trans_pnp(j3d: torch.Tensor, pj2d: torch.Tensor, focal_length: float = 1265.0, img_size: float = 512.0,
+                  n_dev: Optional[torch.Tensor] = None, return_inliers: bool = False):
+    """(n,21,3), (n,21,2) -> (n,3) camera translation as the reference's cv2.solvePnPRansac(EPNP,
+    reprojectionError=20, iterationsCount=100) computes it, on the device; with ``return_inliers`` also the (n,)
+    int32 inlier bitmask over the 21 joints (0 where the result is the least squares or (-1,-1,-1))."""
+    dev = L.require_cuda(j3d, pj2d, n_dev)
+    n = j3d.shape[0]
+    out = torch.empty(n, 3, device=j3d.device)
+    inl = torch.empty(n, dtype=torch.int32, device=j3d.device) if return_inliers else None
+    if n:
+        with L.on(dev):
+            L.check(L.load().acr_b200_cam_trans_pnp(L.ptr(j3d.contiguous().float()), L.ptr(pj2d.contiguous().float()),
+                                                    L.ptr(n_dev), n, float(focal_length), float(img_size), L.ptr(out),
+                                                    L.ptr(inl), L.current_stream(dev)), "cam_trans_pnp")
+    return (out, inl) if return_inliers else out
+
+
+def cam_trans_mode(mode: str, j3d: torch.Tensor, pj2d: torch.Tensor, focal_length: float = 1265.0,
+                   img_size: float = 512.0, n_dev: Optional[torch.Tensor] = None) -> Optional[torch.Tensor]:
+    """``args().cam_trans_mode`` dispatch: 'lstsq' -> cam_trans, 'pnp' -> cam_trans_pnp, anything else
+    ('none') -> None."""
+    if mode == "lstsq":
+        return cam_trans(j3d, pj2d, focal_length, img_size, n_dev=n_dev)
+    if mode == "pnp":
+        return cam_trans_pnp(j3d, pj2d, focal_length, img_size, n_dev=n_dev)
+    return None
+
+
 class OneEuroState:
     """Device-side history of the temporal filter (one bank per hand type); zero = no history."""
 

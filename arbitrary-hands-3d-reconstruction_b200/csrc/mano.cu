@@ -13,6 +13,7 @@
 // once per CTA from L2 (coalesced, [k][c][v] layout) and applies them to all HG hands from
 // registers, with the pose-map coefficients broadcast from shared memory as float4.
 #include "common.cuh"
+#include "cam_trans.cuh"
 #include "rotation.cuh"
 
 namespace acr {
@@ -498,37 +499,14 @@ __global__ void gather_wait_kernel(const unsigned long long* flags, const unsign
   if ((int)threadIdx.x < world) wait_flag_ge(flags + threadIdx.x, *step_dev);
 }
 
-// estimate_translation_np (acr/utils.py:430-472) for one hand per thread, fp64 like the numpy original:
-// rows [f,0,cx-u | (u-cx)*Z - f*X] and [0,f,cy-v | (v-cy)*Z - f*Y] of every usable joint, normal equations.
+// estimate_translation_np for one hand per thread (cam_trans.cuh)
 __global__ void cam_trans_kernel(const float* __restrict__ j3d, const float* __restrict__ pj2d,
                                  const int32_t* __restrict__ n_dev, int n_max, float focal, float img_size,
                                  float* __restrict__ out) {
   const int n = n_dev ? min(*n_dev, n_max) : n_max;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  const double f = focal, c0 = (double)(img_size * 0.5f);
-  double A00 = 0, A01 = 0, A02 = 0, A11 = 0, A12 = 0, A22 = 0, b0 = 0, b1 = 0, b2 = 0;
-  int used = 0;
-  for (int j = 0; j < 21; ++j) {
-    const float X = j3d[((size_t)i * 21 + j) * 3 + 0], Y = j3d[((size_t)i * 21 + j) * 3 + 1], Z = j3d[((size_t)i * 21 + j) * 3 + 2];
-    const float u = (pj2d[((size_t)i * 21 + j) * 2 + 0] + 1.f) * (img_size * 0.5f);
-    const float v = (pj2d[((size_t)i * 21 + j) * 2 + 1] + 1.f) * (img_size * 0.5f);
-    if (!(v > -2.f) || Z == -2.f) continue;   // the reference's "confidence" tests (acr/utils.py:489-492)
-    ++used;
-    const double qx = c0 - (double)u, qy = c0 - (double)v;        // third column of the two rows
-    const double cx = ((double)u - c0) * (double)Z - f * (double)X, cy = ((double)v - c0) * (double)Z - f * (double)Y;
-    A00 += f * f; A02 += f * qx; b0 += f * cx;
-    A11 += f * f; A12 += f * qy; b1 += f * cy;
-    A22 += qx * qx + qy * qy; b2 += qx * cx + qy * cy;
-  }
-  float* o = out + (size_t)i * 3;
-  if (used < 4) { o[0] = o[1] = o[2] = -1.f; return; }
-  // symmetric 3x3 solve (A01 = 0): Cramer's rule in fp64
-  const double det = A00 * (A11 * A22 - A12 * A12) - A01 * (A01 * A22 - A12 * A02) + A02 * (A01 * A12 - A11 * A02);
-  const double d0 = b0 * (A11 * A22 - A12 * A12) - A01 * (b1 * A22 - A12 * b2) + A02 * (b1 * A12 - A11 * b2);
-  const double d1 = A00 * (b1 * A22 - A12 * b2) - b0 * (A01 * A22 - A12 * A02) + A02 * (A01 * b2 - b1 * A02);
-  const double d2 = A00 * (A11 * b2 - b1 * A12) - A01 * (A01 * b2 - b1 * A02) + b0 * (A01 * A12 - A11 * A02);
-  o[0] = (float)(d0 / det); o[1] = (float)(d1 / det); o[2] = (float)(d2 / det);
+  cam_trans_lstsq(j3d + (size_t)i * 63, pj2d + (size_t)i * 42, focal, img_size, out + (size_t)i * 3);
 }
 
 __global__ void rodrigues_kernel(const float* __restrict__ aa, int n, float* __restrict__ out) {

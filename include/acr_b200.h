@@ -159,6 +159,20 @@ int acr_b200_mano_layer_backward(const float* model, int side, const float* pose
 int acr_b200_cam_trans(const float* j3d, const float* pj2d, const int32_t* n_dev, int n_max, float focal_length,
                        float img_size, float* cam_trans, void* stream);
 
+/* Camera translation of every hand as the reference computes it: cv2.solvePnPRansac(SOLVEPNP_EPNP,
+ * reprojectionError=20, iterationsCount=100) with K = [f 0 img_size/2; 0 f img_size/2; 0 0 1] on the usable
+ * joints (the tests of acr_b200_cam_trans), in fp64 on the device, one warp per hand.  OpenCV's deterministic
+ * RANSAC (its RNG, 5-point EPnP hypotheses, fp32 reprojection test) and the final EPnP on all inliers.
+ *   fewer than 4 usable joints  -> (-1,-1,-1), as acr_b200_cam_trans;
+ *   exactly 4                   -> acr_b200_cam_trans's least squares (OpenCV would run P3P: a deviation);
+ *   exactly 5                   -> one EPnP, every joint an inlier (OpenCV skips RANSAC there);
+ *   no RANSAC consensus         -> acr_b200_cam_trans's least squares (the reference's except-branch).
+ * inlier_mask (n) int32, optional (NULL skips it): bit j set iff joint j is an inlier of the final fit; 0 where
+ * the result is the least squares or (-1,-1,-1).  n_dev as in acr_b200_mano_forward; rows >= *n_dev are not
+ * written.  No allocation, no host synchronisation, no atomics: graph-capturable.                       */
+int acr_b200_cam_trans_pnp(const float* j3d, const float* pj2d, const int32_t* n_dev, int n_max, float focal_length,
+                           float img_size, float* cam_trans, int32_t* inlier_mask, void* stream);
+
 /* Frame pre-processing on the device (SURVEY.md 8f-2): n BGR frames (n,H,W,3) -> RGB, white (255) pad to a
  * `side` x `side` square (pad_t rows above, pad_l columns left), bicubic resize to out_size x out_size.
  * Replaces img_preprocess / process_image_ori / image_pad_white_bg + cv2.resize(INTER_CUBIC)
