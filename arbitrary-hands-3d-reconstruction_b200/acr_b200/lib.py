@@ -20,7 +20,7 @@ CONV_DECONV = 32      # ACR_CONV_DECONV flag bit (shift[0]) of a CONV op
 CONV_BLOCK = 64       # ACR_CONV_BLOCK: this conv and the next are one BasicBlock, run as one launch
 CONV_BLOCK_MID = 128  # ACR_CONV_BLOCK_MID: the fused launch also writes the block's intermediate
 DT_BF16, DT_F16, DT_F32, DT_U8 = 0, 1, 2, 3
-POSE_AXISANG, POSE_ROTMAT = 0, 1   # ACR_B200_POSE_*: pose input of acr_b200_mano_layer_forward / _backward
+POSE_AXISANG, POSE_ROTMAT = 0, 1   # ACR_B200_POSE_*: pose input of acr_b200_mano_layer_forward / _backward / _jvp
 
 
 class AcrB200Error(RuntimeError):
@@ -63,7 +63,7 @@ _lib: Optional[C.CDLL] = None
 EXPORTS = ["acr_b200_last_error", "acr_b200_version", "acr_b200_mano_model_floats", "acr_b200_mano_pack_model",
            "acr_b200_mano_forward", "acr_b200_mano_forward_gather", "acr_b200_gather_wait",
            "acr_b200_mano_backward_workspace_floats", "acr_b200_mano_backward", "acr_b200_mano_layer_forward",
-           "acr_b200_mano_layer_backward", "acr_b200_cam_trans", "acr_b200_cam_trans_pnp", "acr_b200_preprocess", "acr_b200_one_euro_state_floats", "acr_b200_one_euro_smooth", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse",
+           "acr_b200_mano_layer_backward", "acr_b200_mano_layer_jvp", "acr_b200_cam_trans", "acr_b200_cam_trans_pnp", "acr_b200_preprocess", "acr_b200_one_euro_state_floats", "acr_b200_one_euro_smooth", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse",
            "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_profile_ops", "acr_b200_plan_num_launches", "acr_b200_plan_op_launch", "acr_b200_plan_destroy",
            "acr_b200_run_op", "acr_b200_pack_conv"]
 
@@ -91,6 +91,7 @@ def load() -> C.CDLL:
     lib.acr_b200_mano_backward.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.acr_b200_mano_layer_forward.argtypes = [vp, i32, vp, i32, vp, i32, i32, i32, vp, vp, vp, vp]
     lib.acr_b200_mano_layer_backward.argtypes = [vp, i32, vp, i32, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.acr_b200_mano_layer_jvp.argtypes = [vp, i32, vp, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.acr_b200_cam_trans.argtypes = [vp, vp, vp, i32, f32, f32, vp, vp]
     lib.acr_b200_cam_trans_pnp.argtypes = [vp, vp, vp, i32, f32, f32, vp, vp, vp]
     lib.acr_b200_preprocess.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp]

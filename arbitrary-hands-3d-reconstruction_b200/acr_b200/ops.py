@@ -142,6 +142,36 @@ def mano_layer_backward(model: torch.Tensor, side: int, pose: torch.Tensor, pose
     return dpose, dbetas
 
 
+def mano_layer_jvp(model: torch.Tensor, side: int, pose: torch.Tensor, pose_mode: int, betas: torch.Tensor,
+                   center_idx: Optional[int], root_palm: bool, tpose: Optional[torch.Tensor],
+                   tbetas: Optional[torch.Tensor], want_verts: bool = True):
+    """Forward-mode derivative of ``mano_layer_forward``: ``tpose`` (T, n, *pose.shape[1:]) and ``tbetas`` (T, n, 10)
+    are T tangents per hand (None is zero) -> (tverts (T,n,778,3) or None, tjoints (T,n,21,3), tcenter (T,n,1,3)).
+    Without ``want_verts`` the kernel computes the joints only (no vertex pass)."""
+    dev = L.require_cuda(model, pose, betas, tpose, tbetas)
+    n = pose.shape[0]
+    T = (tpose if tpose is not None else tbetas).shape[0] if (tpose is not None or tbetas is not None) else 0
+    pose = pose.contiguous().float()
+    betas = betas.contiguous().float()
+    tpose, tbetas = [None if t is None else t.contiguous().float() for t in (tpose, tbetas)]
+    assert tpose is None or tpose.shape == (T,) + tuple(pose.shape)
+    assert tbetas is None or tbetas.shape == (T, n, 10)
+    idle = T == 0 or n == 0 or (tpose is None and tbetas is None)
+    alloc = torch.zeros if idle else torch.empty     # the kernel writes every element
+    tverts = alloc(T, n, 778, 3, device=dev) if want_verts else None
+    tjoints, tcenter = alloc(T, n, 21, 3, device=dev), alloc(T, n, 1, 3, device=dev)
+    if idle:
+        return tverts, tjoints, tcenter
+    lib = L.load()
+    with L.on(dev):
+        rc = lib.acr_b200_mano_layer_jvp(L.ptr(model), int(side), L.ptr(pose), int(pose_mode), L.ptr(betas), n,
+                                         -1 if center_idx is None else int(center_idx), int(bool(root_palm)), T,
+                                         L.ptr(tpose), L.ptr(tbetas), None, None, None, L.ptr(tverts), L.ptr(tjoints),
+                                         L.ptr(tcenter), L.current_stream(dev))
+    L.check(rc, "mano_layer_jvp")
+    return tverts, tjoints, tcenter
+
+
 def cam_trans(j3d: torch.Tensor, pj2d: torch.Tensor, focal_length: float = 1265.0, img_size: float = 512.0,
               n_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
     """(n,21,3), (n,21,2) -> (n,3) camera translation (closed-form least squares on the device)."""

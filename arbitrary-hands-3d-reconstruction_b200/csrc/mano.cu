@@ -885,6 +885,441 @@ __global__ void __launch_bounds__(VPB) mano_layer_backward_chain_kernel(const Ma
   mano_backward_chain_body<kPose, kPalm>(p);
 }
 
+// --------------------------------------------------------------------------------------------------- MANO JVP
+// Forward-mode derivative of acr_b200_mano_layer_forward: NT tangents of each hand per CTA, no atomics, and every
+// tangent runs the same instructions in the same order whatever its slot in a tile, so its result does not depend on
+// n_tan or on which tangents share its CTA.
+//   phase 1 (thread = (hand, joint)): the primal transforms (rebuild_transforms), then per tangent the rotation
+//     tangent dR_j, dJ = JS . dbeta, the chain tangents dG (three levels per finger) and dA_j, all in shared memory;
+//   phase 2, full form (thread = vertex): d v_posed = sum_k dirs_k dpm_k, d vert = dT [v_posed; 1] + T d v_posed;
+//   phase 2, joints-only form (thread = (hand, tip or palm vertex)): the same for the five tips and the palm only.
+constexpr int NT = 4;                 // tangents per CTA (the tangent arrays below take 51.8 KB of shared memory)
+constexpr int JCOLS = NT * HG;        // columns (tangent, hand) of the blend-row tangents, [k][t * HG + h]
+constexpr int TS_DPM = 0;                             // [NK][JCOLS]         d pm: dR_j (j >= 1) and dbeta
+constexpr int TS_DG = TS_DPM + NK * JCOLS;            // [NT][HG][16][12]    dG, then dA in place
+constexpr int TS_DJ = TS_DG + NT * HG * 16 * 12;      // [NT][HG][16][3]     d rest joints
+constexpr int TS_DR0 = TS_DJ + NT * HG * 16 * 3;      // [NT][HG][9]         dR of the root
+constexpr int TS_DCTR = TS_DR0 + NT * HG * 9;         // [NT][HG][3]         d centre
+constexpr int TS_PALM = TS_DCTR + NT * HG * 3;        // [NT + 1][HG][2][3]  palm vertices (slot NT: the primal)
+constexpr int TS_FLOATS = TS_PALM + (NT + 1) * HG * 6;
+constexpr size_t JVP_DYN_SMEM = (size_t)TS_FLOATS * sizeof(float);
+static_assert(TS_DG % 4 == 0 && JCOLS % 16 == 0, "16-byte shared loads");
+
+struct ManoJvpParams {
+  const float* model;
+  int side;
+  const float* poses;
+  const float* betas;
+  int n;
+  int center_src;
+  int n_tan;
+  const float* tposes;   // (n_tan, n, 48) or (n_tan, n, 16, 3, 3), or null (zero)
+  const float* tbetas;   // (n_tan, n, 10), or null
+  float* verts;
+  float* joints;
+  float* center;
+  float* tverts;         // (n_tan, n, 778, 3)
+  float* tjoints;        // (n_tan, n, 21, 3)
+  float* tcenter;        // (n_tan, n, 3)
+};
+
+// fingertip vertex of slot 0..4 (manolayer.py:244-247)
+__device__ __forceinline__ int tip_vertex(int s, int side) {
+  return s == 0 ? 745 : s == 1 ? 317 : s == 2 ? (side ? 444 : 445) : s == 3 ? 556 : 673;
+}
+
+// a vertex and its tangent from the skinning transform T, its tangent dT, v_posed and d v_posed; explicit FMAs, so
+// both JVP forms produce the same bits
+__device__ __forceinline__ float vert_row(const float (&T)[12], int r, const float (&vp)[3], float ctr) {
+  return fmaf(T[r * 4 + 2], vp[2], fmaf(T[r * 4 + 1], vp[1], fmaf(T[r * 4 + 0], vp[0], T[r * 4 + 3]))) - ctr;
+}
+__device__ __forceinline__ float tan_row(const float (&T)[12], const float (&dT)[12], int r, const float (&vp)[3],
+                                         const float (&dvp)[3], float dctr) {
+  float a = dT[r * 4 + 3];
+  a = fmaf(dT[r * 4 + 0], vp[0], a); a = fmaf(dT[r * 4 + 1], vp[1], a); a = fmaf(dT[r * 4 + 2], vp[2], a);
+  a = fmaf(T[r * 4 + 0], dvp[0], a); a = fmaf(T[r * 4 + 1], dvp[1], a); a = fmaf(T[r * 4 + 2], dvp[2], a);
+  return a - dctr;
+}
+
+// blend-row order of blend_vertex: the shape rows first
+__device__ __forceinline__ int blend_row(int kk) { return (kk < 10) ? 135 + kk : kk - 10; }
+
+// d v_posed of vertex column vc for 2 tangents x HG hands (columns c0 .. c0+15 of s_dpm), from zero
+__device__ __forceinline__ void blend_tangents(const float* __restrict__ m, int vc, const float* s_dpm, int c0,
+                                               float (&acc)[2 * HG][3]) {
+  const float* __restrict__ dirs = m + OFF_DIRS;
+  unsigned long long acc2[HG][3];
+#pragma unroll
+  for (int i = 0; i < HG; ++i) acc2[i][0] = acc2[i][1] = acc2[i][2] = 0ull;   // +0.f pairs
+#pragma unroll 5
+  for (int kk = 0; kk < NK; ++kk) {
+    const int k = blend_row(kk);
+    const float d0 = __ldg(dirs + ((size_t)k * 3 + 0) * NVP + vc);
+    const float d1 = __ldg(dirs + ((size_t)k * 3 + 1) * NVP + vc);
+    const float d2 = __ldg(dirs + ((size_t)k * 3 + 2) * NVP + vc);
+    const float4* row = reinterpret_cast<const float4*>(s_dpm + k * JCOLS + c0);
+    const unsigned long long D0 = pk2(d0, d0), D1 = pk2(d1, d1), D2 = pk2(d2, d2);
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const float4 x = row[q];
+      const unsigned long long P0 = pk2(x.x, x.y), P1 = pk2(x.z, x.w);
+      ffma2(acc2[2 * q][0], D0, P0); ffma2(acc2[2 * q][1], D1, P0); ffma2(acc2[2 * q][2], D2, P0);
+      ffma2(acc2[2 * q + 1][0], D0, P1); ffma2(acc2[2 * q + 1][1], D1, P1); ffma2(acc2[2 * q + 1][2], D2, P1);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < HG; ++i)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) unpk2(acc2[i][c], acc[2 * i][c], acc[2 * i + 1][c]);
+}
+
+// Phase 1 of both JVP forms.  `writer`: this CTA writes the kinematic joints and the centre (tangents of its tile;
+// the primal too when it is tangent tile 0).  Ends synchronised, with dA_j in place of dG_j.
+template <int kPose, bool kPalm>
+__device__ __forceinline__ void jvp_transforms(const ManoJvpParams& p, bool writer, float (*s_pm)[HG],
+                                               float (*s_A)[16][12], float (*s_R)[16][9], float (*s_J)[16][3],
+                                               float (*s_G)[16][12], float (*s_ctr)[3], float* s_t) {
+  const int g0 = blockIdx.x * HG, tile0 = blockIdx.y * NT;
+  const int t = threadIdx.x, h = t >> 4, j = t & 15;
+  const int hand = g0 + h;
+  const bool hvalid = hand < p.n;
+  const float* __restrict__ m = p.model;
+  rebuild_transforms<true, kPose>(hvalid, m, p.poses, p.betas, hand, h, j, p.center_src, s_pm, s_A, s_R, s_J, s_G,
+                                  s_ctr);
+  if (writer && hvalid && blockIdx.y == 0) {
+    const float* G = s_G[h][j];
+    if (p.joints && !(kPalm && j == 0)) {
+      float* o = p.joints + ((size_t)hand * 21 + c_joint_inv[j]) * 3;
+      o[0] = G[3] - s_ctr[h][0]; o[1] = G[7] - s_ctr[h][1]; o[2] = G[11] - s_ctr[h][2];
+    }
+    if (j < 3 && p.center) p.center[(size_t)hand * 3 + j] = s_ctr[h][j];
+  }
+  float* s_dpm = s_t + TS_DPM;
+  float* s_dG = s_t + TS_DG;
+  float* s_dJ = s_t + TS_DJ;
+  float* s_dR0 = s_t + TS_DR0;
+  float* s_dctr = s_t + TS_DCTR;
+  // ---- per tangent: dR_j, dJ_j = JS_j . dbeta, and the blend-row tangents
+  So3ProjectJvp proj;
+  if constexpr (kPose == POSE_ROTMAT) {
+    if (hvalid && p.tposes) proj.setup(p.poses + ((size_t)hand * 16 + j) * 9);
+  }
+#pragma unroll 1
+  for (int u = 0; u < NT; ++u) {
+    const int tt = tile0 + u;
+    const bool valid = hvalid && tt < p.n_tan;
+    const size_t row = (size_t)tt * p.n + hand;
+    const int col = u * HG + h;
+    float dR[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+    if (valid && p.tposes) {
+      if constexpr (kPose == POSE_ROTMAT) {
+        proj.apply(p.tposes + (row * 16 + j) * 9, dR);
+      } else {
+        const float* ps = p.poses + (size_t)hand * 48 + j * 3;
+        rodrigues_jvp(ps[0] + m[OFF_HM + j * 3 + 0], ps[1] + m[OFF_HM + j * 3 + 1], ps[2] + m[OFF_HM + j * 3 + 2],
+                      p.tposes + row * 48 + j * 3, dR);
+      }
+    }
+    float dJ[3] = {0.f, 0.f, 0.f};
+    if (valid && p.tbetas) {
+      const float* db = p.tbetas + row * 10;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float* js = m + OFF_JS + (j * 3 + c) * 10;
+        float a = 0.f;
+#pragma unroll
+        for (int k = 0; k < 10; ++k) a = fmaf(js[k], db[k], a);
+        dJ[c] = a;
+      }
+      if (j < 10) s_dpm[(135 + j) * JCOLS + col] = db[j];
+    } else if (j < 10) {
+      s_dpm[(135 + j) * JCOLS + col] = 0.f;
+    }
+#pragma unroll
+    for (int e = 0; e < 9; ++e) {
+      if (j >= 1) s_dpm[((j - 1) * 9 + e) * JCOLS + col] = dR[e];
+      else s_dR0[col * 9 + e] = dR[e];
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s_dJ[(col * 16 + j) * 3 + c] = dJ[c];
+    if (j < 3) s_dctr[col * 3 + j] = 0.f;
+  }
+  __syncthreads();
+  // ---- chain tangents: task = (tangent, hand, finger 0..4 or the root 5)
+#pragma unroll 1
+  for (int task = t; task < NT * HG * 6; task += VPB) {
+    const int col = task / 6, f = task - col * 6, hh = col % HG;
+    const float* dJ = s_dJ + col * 48;
+    float* dG = s_dG + col * 192;
+    float dP[12];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      dP[r * 4 + 0] = s_dR0[col * 9 + r * 3 + 0]; dP[r * 4 + 1] = s_dR0[col * 9 + r * 3 + 1];
+      dP[r * 4 + 2] = s_dR0[col * 9 + r * 3 + 2]; dP[r * 4 + 3] = dJ[r];
+    }
+    if (f == 5) {
+#pragma unroll
+      for (int e = 0; e < 12; ++e) dG[e] = dP[e];
+      if (p.center_src == 0) { s_dctr[col * 3 + 0] = dP[3]; s_dctr[col * 3 + 1] = dP[7]; s_dctr[col * 3 + 2] = dP[11]; }
+      continue;
+    }
+    int parent = 0;
+#pragma unroll
+    for (int lev = 0; lev < 3; ++lev) {
+      const int idx = 3 * f + 1 + lev;
+      const float* Gp = s_G[hh][parent];
+      const float* Rl = s_R[hh][idx];
+      float dRl[9];
+#pragma unroll
+      for (int e = 0; e < 9; ++e) dRl[e] = s_dpm[((idx - 1) * 9 + e) * JCOLS + col];
+      const float rel[3] = {s_J[hh][idx][0] - s_J[hh][parent][0], s_J[hh][idx][1] - s_J[hh][parent][1],
+                            s_J[hh][idx][2] - s_J[hh][parent][2]};
+      const float drel[3] = {dJ[idx * 3 + 0] - dJ[parent * 3 + 0], dJ[idx * 3 + 1] - dJ[parent * 3 + 1],
+                             dJ[idx * 3 + 2] - dJ[parent * 3 + 2]};
+      // N = Gp [Rl | rel] + [0 | t_p]:  dN = dGp [Rl | rel] + Gp [dRl | drel] + [0 | dt_p]
+      float dN[12];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c)
+          dN[r * 4 + c] = dP[r * 4 + 0] * Rl[0 * 3 + c] + dP[r * 4 + 1] * Rl[1 * 3 + c] + dP[r * 4 + 2] * Rl[2 * 3 + c] +
+                          Gp[r * 4 + 0] * dRl[0 * 3 + c] + Gp[r * 4 + 1] * dRl[1 * 3 + c] + Gp[r * 4 + 2] * dRl[2 * 3 + c];
+        dN[r * 4 + 3] = dP[r * 4 + 0] * rel[0] + dP[r * 4 + 1] * rel[1] + dP[r * 4 + 2] * rel[2] +
+                        Gp[r * 4 + 0] * drel[0] + Gp[r * 4 + 1] * drel[1] + Gp[r * 4 + 2] * drel[2] + dP[r * 4 + 3];
+      }
+#pragma unroll
+      for (int e = 0; e < 12; ++e) { dP[e] = dN[e]; dG[idx * 12 + e] = dN[e]; }
+      if (idx == p.center_src) { s_dctr[col * 3 + 0] = dN[3]; s_dctr[col * 3 + 1] = dN[7]; s_dctr[col * 3 + 2] = dN[11]; }
+      parent = idx;
+    }
+  }
+  __syncthreads();
+  // ---- kinematic joint and centre tangents, then dA_j = [dR_g | dt_g - dR_g J_j - R_g dJ_j] in place of dG_j
+#pragma unroll 1
+  for (int u = 0; u < NT; ++u) {
+    const int tt = tile0 + u, col = u * HG + h;
+    float* dG = s_dG + (col * 16 + j) * 12;
+    const float* dJ = s_dJ + (col * 16 + j) * 3;
+    const float* dc = s_dctr + col * 3;
+    if (writer && hvalid && tt < p.n_tan) {
+      const size_t row = (size_t)tt * p.n + hand;
+      if (p.tjoints && !(kPalm && j == 0)) {
+        float* o = p.tjoints + (row * 21 + c_joint_inv[j]) * 3;
+        o[0] = dG[3] - dc[0]; o[1] = dG[7] - dc[1]; o[2] = dG[11] - dc[2];
+      }
+      if (j < 3 && p.tcenter) p.tcenter[row * 3 + j] = dc[j];
+    }
+    const float* G = s_G[h][j];
+    const float* J = s_J[h][j];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+      dG[r * 4 + 3] = dG[r * 4 + 3] - (dG[r * 4 + 0] * J[0] + dG[r * 4 + 1] * J[1] + dG[r * 4 + 2] * J[2]) -
+                      (G[r * 4 + 0] * dJ[0] + G[r * 4 + 1] * dJ[1] + G[r * 4 + 2] * dJ[2]);
+  }
+  __syncthreads();
+}
+
+// palm joint (slot NT: the primal, written by tangent tile 0) from the two staged palm vertices of each hand
+__device__ __forceinline__ void jvp_write_palm(const ManoJvpParams& p, const float* s_palm) {
+  const int g0 = blockIdx.x * HG, tile0 = blockIdx.y * NT;
+  for (int task = threadIdx.x; task < (NT + 1) * HG; task += VPB) {
+    const int u = task / HG, h = task - u * HG, hand = g0 + h;
+    if (hand >= p.n) continue;
+    const float* s = s_palm + task * 6;
+    float* o;
+    if (u == NT) {
+      if (blockIdx.y != 0 || !p.joints) continue;
+      o = p.joints + (size_t)hand * 21 * 3;
+    } else {
+      if (tile0 + u >= p.n_tan || !p.tjoints) continue;
+      o = p.tjoints + ((size_t)(tile0 + u) * p.n + hand) * 21 * 3;
+    }
+    o[0] = (s[0] + s[3]) * 0.5f; o[1] = (s[1] + s[4]) * 0.5f; o[2] = (s[2] + s[5]) * 0.5f;
+  }
+}
+
+// full form: grid (hand groups, tangent tiles, vertex chunks)
+template <int kPose, bool kPalm>
+__global__ void __launch_bounds__(VPB) mano_layer_jvp_kernel(const ManoJvpParams p) {
+  __shared__ __align__(16) float s_pm[NK][HG];
+  __shared__ __align__(16) float s_A[HG][16][12];
+  __shared__ float s_R[HG][16][9];
+  __shared__ float s_J[HG][16][3];
+  __shared__ float s_G[HG][16][12];
+  __shared__ float s_ctr[HG][3];
+  extern __shared__ __align__(16) float s_t[];
+  jvp_transforms<kPose, kPalm>(p, blockIdx.z == 0, s_pm, s_A, s_R, s_J, s_G, s_ctr, s_t);
+  const float* s_dpm = s_t + TS_DPM;
+  const float* s_dA = s_t + TS_DG;
+  const float* s_dctr = s_t + TS_DCTR;
+  float* s_palm = s_t + TS_PALM;
+  const float* __restrict__ m = p.model;
+  const int g0 = blockIdx.x * HG, tile0 = blockIdx.y * NT;
+  const int v = blockIdx.z * VPB + threadIdx.x;
+  const bool vvalid = v < NV;
+  const int vc = vvalid ? v : NVP - 1;
+  float vp[HG][3];
+  blend_vertex(m, vc, s_pm, vp);
+  float w[16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) w[j] = __ldg(m + OFF_W + j * NVP + vc);
+  int tip = -1;
+#pragma unroll
+  for (int s = 0; s < 5; ++s)
+    if (v == tip_vertex(s, p.side)) tip = s;
+  const int palm = (kPalm && v == PALM_VA) ? 0 : (kPalm && v == PALM_VB) ? 1 : -1;
+  // the primal, from tangent tile 0
+  if (blockIdx.y == 0 && (p.verts || p.joints)) {
+#pragma unroll
+    for (int h = 0; h < HG; ++h) {
+      const int hand = g0 + h;
+      if (hand >= p.n) continue;                // block-uniform
+      float T[12];
+      skin_transform(w, s_A[h], T);
+      float x[3];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) x[r] = vert_row(T, r, vp[h], s_ctr[h][r]);
+      if (!vvalid) continue;
+      if (p.verts) {
+        float* o = p.verts + ((size_t)hand * NV + v) * 3;
+        o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+      }
+      if (tip >= 0 && p.joints) {
+        float* o = p.joints + ((size_t)hand * 21 + c_joint_inv[16 + tip]) * 3;
+        o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+      }
+      if (palm >= 0) {
+        float* s = s_palm + (NT * HG + h) * 6 + palm * 3;
+        s[0] = x[0]; s[1] = x[1]; s[2] = x[2];
+      }
+    }
+  }
+  // the tangents, two per pass
+#pragma unroll 1
+  for (int pass = 0; pass < NT / 2; ++pass) {
+    float dvp[2 * HG][3];
+    blend_tangents(m, vc, s_dpm, pass * 2 * HG, dvp);
+#pragma unroll
+    for (int h = 0; h < HG; ++h) {
+      const int hand = g0 + h;
+      if (hand >= p.n) continue;                // block-uniform
+      float T[12];
+      skin_transform(w, s_A[h], T);
+#pragma unroll
+      for (int q = 0; q < 2; ++q) {
+        const int u = pass * 2 + q, tt = tile0 + u, col = u * HG + h;
+        if (tt >= p.n_tan) continue;            // block-uniform
+        float dT[12];
+        skin_transform(w, reinterpret_cast<const float(*)[12]>(s_dA + col * 192), dT);
+        float x[3];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) x[r] = tan_row(T, dT, r, vp[h], dvp[q * HG + h], s_dctr[col * 3 + r]);
+        if (!vvalid) continue;
+        const size_t row = (size_t)tt * p.n + hand;
+        if (p.tverts) {
+          float* o = p.tverts + (row * NV + v) * 3;
+          o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+        }
+        if (tip >= 0 && p.tjoints) {
+          float* o = p.tjoints + (row * 21 + c_joint_inv[16 + tip]) * 3;
+          o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+        }
+        if (palm >= 0) {
+          float* s = s_palm + col * 6 + palm * 3;
+          s[0] = x[0]; s[1] = x[1]; s[2] = x[2];
+        }
+      }
+    }
+  }
+  if constexpr (kPalm) {
+    __syncthreads();
+    if (blockIdx.z == 0) jvp_write_palm(p, s_palm);
+  }
+}
+
+// joints-only form: grid (hand groups, tangent tiles); thread (hand, s) takes tip s < 5 or palm vertex s - 5
+template <int kPose, bool kPalm>
+__global__ void __launch_bounds__(VPB) mano_layer_jvp_joints_kernel(const ManoJvpParams p) {
+  __shared__ __align__(16) float s_pm[NK][HG];
+  __shared__ __align__(16) float s_A[HG][16][12];
+  __shared__ float s_R[HG][16][9];
+  __shared__ float s_J[HG][16][3];
+  __shared__ float s_G[HG][16][12];
+  __shared__ float s_ctr[HG][3];
+  extern __shared__ __align__(16) float s_t[];
+  jvp_transforms<kPose, kPalm>(p, true, s_pm, s_A, s_R, s_J, s_G, s_ctr, s_t);
+  const float* s_dpm = s_t + TS_DPM;
+  const float* s_dA = s_t + TS_DG;
+  const float* s_dctr = s_t + TS_DCTR;
+  float* s_palm = s_t + TS_PALM;
+  const float* __restrict__ m = p.model;
+  const int g0 = blockIdx.x * HG, tile0 = blockIdx.y * NT;
+  const int h = threadIdx.x >> 4, s = threadIdx.x & 15, hand = g0 + h;
+  if (s < (kPalm ? 7 : 5) && hand < p.n) {
+    const int v = s < 5 ? tip_vertex(s, p.side) : (s == 5 ? PALM_VA : PALM_VB);
+    const float* __restrict__ dirs = m + OFF_DIRS;
+    // v_posed and its NT tangents in blend_vertex's / blend_tangents' order of rows and operations
+    float vp[3] = {m[OFF_VT + 0 * NVP + v], m[OFF_VT + 1 * NVP + v], m[OFF_VT + 2 * NVP + v]};
+    float dvp[NT][3];
+#pragma unroll
+    for (int u = 0; u < NT; ++u) dvp[u][0] = dvp[u][1] = dvp[u][2] = 0.f;
+#pragma unroll 5
+    for (int kk = 0; kk < NK; ++kk) {
+      const int k = blend_row(kk);
+      const float d[3] = {__ldg(dirs + ((size_t)k * 3 + 0) * NVP + v), __ldg(dirs + ((size_t)k * 3 + 1) * NVP + v),
+                          __ldg(dirs + ((size_t)k * 3 + 2) * NVP + v)};
+      const float c = s_pm[k][h];
+#pragma unroll
+      for (int r = 0; r < 3; ++r) vp[r] = fmaf(d[r], c, vp[r]);
+#pragma unroll
+      for (int u = 0; u < NT; ++u) {
+        const float dc = s_dpm[k * JCOLS + u * HG + h];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) dvp[u][r] = fmaf(d[r], dc, dvp[u][r]);
+      }
+    }
+    float w[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) w[j] = __ldg(m + OFF_W + j * NVP + v);
+    float T[12];
+    skin_transform(w, s_A[h], T);
+    float x[3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r) x[r] = vert_row(T, r, vp, s_ctr[h][r]);
+    if (s < 5) {
+      if (blockIdx.y == 0 && p.joints) {
+        float* o = p.joints + ((size_t)hand * 21 + c_joint_inv[16 + s]) * 3;
+        o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+      }
+    } else {
+      float* o = s_palm + (NT * HG + h) * 6 + (s - 5) * 3;
+      o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+    }
+#pragma unroll
+    for (int u = 0; u < NT; ++u) {
+      const int tt = tile0 + u, col = u * HG + h;
+      if (tt >= p.n_tan) break;
+      float dT[12];
+      skin_transform(w, reinterpret_cast<const float(*)[12]>(s_dA + col * 192), dT);
+#pragma unroll
+      for (int r = 0; r < 3; ++r) x[r] = tan_row(T, dT, r, vp, dvp[u], s_dctr[col * 3 + r]);
+      if (s < 5) {
+        if (p.tjoints) {
+          float* o = p.tjoints + (((size_t)tt * p.n + hand) * 21 + c_joint_inv[16 + s]) * 3;
+          o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+        }
+      } else {
+        float* o = s_palm + col * 6 + (s - 5) * 3;
+        o[0] = x[0]; o[1] = x[1]; o[2] = x[2];
+      }
+    }
+  }
+  if constexpr (kPalm) {
+    __syncthreads();
+    jvp_write_palm(p, s_palm);
+  }
+}
+
 }  // namespace acr
 
 using namespace acr;
@@ -1126,6 +1561,47 @@ extern "C" int acr_b200_mano_layer_backward(const float* model, int side, const 
     return root_palm ? launch_layer_backward<POSE_ROTMAT, true>(p, partials, s)
                      : launch_layer_backward<POSE_ROTMAT, false>(p, partials, s);
   return launch_layer_backward<POSE_AXISANG, true>(p, partials, s);
+}
+
+template <int kPose, bool kPalm>
+static int launch_layer_jvp(const ManoJvpParams& p, bool full, cudaStream_t s) {
+  const dim3 grid(ceil_div(p.n, HG), ceil_div(max(p.n_tan, 1), NT), full ? NCHUNK : 1);
+  if (full) {
+    static unsigned long long smem_done = 0;
+    ACR_CHECK_CUDA(ensure_dynamic_smem(mano_layer_jvp_kernel<kPose, kPalm>, (int)JVP_DYN_SMEM, &smem_done));
+    mano_layer_jvp_kernel<kPose, kPalm><<<grid, VPB, JVP_DYN_SMEM, s>>>(p);
+  } else {
+    static unsigned long long smem_done = 0;
+    ACR_CHECK_CUDA(ensure_dynamic_smem(mano_layer_jvp_joints_kernel<kPose, kPalm>, (int)JVP_DYN_SMEM, &smem_done));
+    mano_layer_jvp_joints_kernel<kPose, kPalm><<<grid, VPB, JVP_DYN_SMEM, s>>>(p);
+  }
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}
+
+extern "C" int acr_b200_mano_layer_jvp(const float* model, int side, const float* pose, int pose_mode,
+                                       const float* betas, int n, int center_idx, int root_palm, int n_tan,
+                                       const float* tpose, const float* tbetas, float* verts, float* joints,
+                                       float* center, float* tverts, float* tjoints, float* tcenter, void* stream) {
+  ACR_CHECK_ARG(n >= 0, "mano_layer_jvp: n < 0");
+  ACR_CHECK_ARG(n_tan >= 0, "mano_layer_jvp: n_tan < 0");
+  if (n == 0) return ACR_B200_OK;
+  ACR_CHECK_ARG(model && pose && betas, "mano_layer_jvp: model / pose / betas are null");
+  ACR_CHECK_ARG(n_tan <= 65535 * NT, "mano_layer_jvp: n_tan > %d", 65535 * NT);
+  int center_src;
+  if (const int rc = layer_args("mano_layer_jvp", side, pose_mode, center_idx, root_palm, &center_src)) return rc;
+  const bool tangents = n_tan > 0 && (tverts || tjoints || tcenter);
+  if (!tangents && !verts && !joints && !center) return ACR_B200_OK;
+  ManoJvpParams p = {};
+  p.model = model; p.side = side; p.poses = pose; p.betas = betas; p.n = n; p.center_src = center_src;
+  p.n_tan = tangents ? n_tan : 0; p.tposes = tpose; p.tbetas = tbetas;
+  p.verts = verts; p.joints = joints; p.center = center; p.tverts = tverts; p.tjoints = tjoints; p.tcenter = tcenter;
+  // without vertices (primal or tangent) one CTA per hand group and tangent tile: the joints-only form
+  const bool full = verts || tverts;
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (pose_mode == ACR_B200_POSE_ROTMAT)
+    return root_palm ? launch_layer_jvp<POSE_ROTMAT, true>(p, full, s) : launch_layer_jvp<POSE_ROTMAT, false>(p, full, s);
+  return root_palm ? launch_layer_jvp<POSE_AXISANG, true>(p, full, s) : launch_layer_jvp<POSE_AXISANG, false>(p, full, s);
 }
 
 extern "C" int acr_b200_gather_wait(const acr_b200_gather* g, void* stream) {

@@ -72,6 +72,38 @@ __device__ __forceinline__ void rodrigues_vjp(float ax, float ay, float az, cons
   da[2] = sa * dq[3] + dang * (bz / ang);
 }
 
+// Jacobian-vector product of rodrigues(): da (tangent of the axis angle) -> dR (row-major).  The forward-mode twin
+// of rodrigues_vjp, in the same bounded quantities n = a/angle and s/angle, so it is finite at a = 0 as well.
+__device__ __forceinline__ void rodrigues_jvp(float ax, float ay, float az, const float* da, float* dR) {
+  const float bx = ax + 1e-8f, by = ay + 1e-8f, bz = az + 1e-8f;
+  const float ang = sqrtf(bx * bx + by * by + bz * bz);
+  const float nx = ax / ang, ny = ay / ang, nz = az / ang;
+  float s, c;
+  half_angle_sincos<true>(ang, &s, &c);
+  const float q[4] = {c, s * nx, s * ny, s * nz};
+  const float qn = sqrtf(q[0] * q[0] + q[1] * q[1] + q[2] * q[2] + q[3] * q[3]);
+  const float w = q[0] / qn, x = q[1] / qn, y = q[2] / qn, z = q[3] / qn;
+  // q = [cos(ang/2), (s/ang) a]:  d ang = (b/ang) . da,  d(s/ang) a = n (c/2 - s/ang) d ang
+  const float sa = s / ang;
+  const float dang = (bx / ang) * da[0] + (by / ang) * da[1] + (bz / ang) * da[2];
+  const float k = (0.5f * c - sa) * dang;
+  float dq[4] = {-0.5f * s * dang, sa * da[0] + nx * k, sa * da[1] + ny * k, sa * da[2] + nz * k};
+  // q / ||q||
+  const float proj = w * dq[0] + x * dq[1] + y * dq[2] + z * dq[3];
+  const float dw = (dq[0] - w * proj) / qn, dx = (dq[1] - x * proj) / qn;
+  const float dy = (dq[2] - y * proj) / qn, dz = (dq[3] - z * proj) / qn;
+  // quat2mat, differentiated entry by entry
+  dR[0] = 2.f * (w * dw + x * dx - y * dy - z * dz);
+  dR[1] = 2.f * (dx * y + x * dy - dw * z - w * dz);
+  dR[2] = 2.f * (dw * y + w * dy + dx * z + x * dz);
+  dR[3] = 2.f * (dw * z + w * dz + dx * y + x * dy);
+  dR[4] = 2.f * (w * dw - x * dx + y * dy - z * dz);
+  dR[5] = 2.f * (dy * z + y * dz - dw * x - w * dx);
+  dR[6] = 2.f * (dx * z + x * dz - dw * y - w * dy);
+  dR[7] = 2.f * (dw * x + w * dx + dy * z + y * dz);
+  dR[8] = 2.f * (w * dw - x * dx - y * dy + z * dz);
+}
+
 // ------------------------------------------------------------------------------ SO(3) projection (batch_rotprojs)
 // The reference (mano/manolayer.py:436-453) takes the SVD M = U S V^T of every input matrix, forms the orthogonal
 // polar factor Q = U V^T and negates column 2 of Q when det Q < 0.  Here, per thread and in fp64: a fixed-sweep
@@ -206,6 +238,54 @@ __device__ __forceinline__ void so3_project_vjp(const float* __restrict__ Mf, co
     dM[r * 3 + 2] = (float)(Q[r][0] * z1 - Q[r][1] * z0);
   }
 }
+
+// Jacobian-vector product of so3_project(), for several tangents of one matrix.  M = Q P with P = Q^T M symmetric,
+// so dM = dQ P + Q dP with dQ = Q [w]x and dP symmetric: the skew part of X = Q^T dM is that of [w]x P + P [w]x =
+// [((tr P) I - P) w]x, hence w = ((tr P) I - P)^-1 axial(X - X^T) and dR = Q [w]x D.  The same matrix as in the VJP
+// (finite unless two singular values sum to zero, so at exact rotations too); set up once, then apply per tangent.
+struct So3ProjectJvp {
+  double Q[3][3];
+  double c00, c01, c02, c11, c12, c22;   // adjugate of (tr P) I - P (symmetrised), divided by its determinant
+  bool flip;
+
+  __device__ __forceinline__ void setup(const float* __restrict__ Mf) {
+    polar_factor(Mf, Q, flip);
+    double P[3][3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        P[r][c] = Q[0][r] * (double)Mf[0 * 3 + c] + Q[1][r] * (double)Mf[1 * 3 + c] + Q[2][r] * (double)Mf[2 * 3 + c];
+    const double tr = P[0][0] + P[1][1] + P[2][2];
+    const double a00 = tr - P[0][0], a11 = tr - P[1][1], a22 = tr - P[2][2];
+    const double a01 = -0.5 * (P[0][1] + P[1][0]), a02 = -0.5 * (P[0][2] + P[2][0]), a12 = -0.5 * (P[1][2] + P[2][1]);
+    c00 = a11 * a22 - a12 * a12; c01 = a02 * a12 - a01 * a22; c02 = a01 * a12 - a02 * a11;
+    c11 = a00 * a22 - a02 * a02; c12 = a01 * a02 - a00 * a12; c22 = a00 * a11 - a01 * a01;
+    const double inv = 1.0 / (a00 * c00 + a01 * c01 + a02 * c02);
+    c00 *= inv; c01 *= inv; c02 *= inv; c11 *= inv; c12 *= inv; c22 *= inv;
+  }
+
+  // dM (tangent of M, row-major, fp32) -> dR (row-major, fp32)
+  __device__ __forceinline__ void apply(const float* __restrict__ dMf, float* __restrict__ dR) const {
+    double X[3][3];
+#pragma unroll
+    for (int r = 0; r < 3; ++r)
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        X[r][c] = Q[0][r] * (double)dMf[0 * 3 + c] + Q[1][r] * (double)dMf[1 * 3 + c] + Q[2][r] * (double)dMf[2 * 3 + c];
+    const double k0 = X[2][1] - X[1][2], k1 = X[0][2] - X[2][0], k2 = X[1][0] - X[0][1];
+    const double z0 = c00 * k0 + c01 * k1 + c02 * k2;
+    const double z1 = c01 * k0 + c11 * k1 + c12 * k2;
+    const double z2 = c02 * k0 + c12 * k1 + c22 * k2;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      dR[r * 3 + 0] = (float)(Q[r][1] * z2 - Q[r][2] * z1);
+      dR[r * 3 + 1] = (float)(Q[r][2] * z0 - Q[r][0] * z2);
+      const double d2 = Q[r][0] * z1 - Q[r][1] * z0;
+      dR[r * 3 + 2] = (float)(flip ? -d2 : d2);
+    }
+  }
+};
 
 // rotation_matrix_to_angle_axis (acr/utils.py:334-360) of a row-major 3x3 (not necessarily orthonormal)
 // matrix: 4-case quaternion on the TRANSPOSED matrix (:862-906), atan2 form (:803-823), NaN -> 0.

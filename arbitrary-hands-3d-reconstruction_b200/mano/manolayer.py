@@ -9,8 +9,12 @@ enabled and pose or betas requiring grad, the kernel runs inside ``_ManoFunction
 ``acr_b200_mano_backward``.  Otherwise the forward makes exactly the launch it makes without autograd.
 
 Rotation-matrix joints (``use_pca=False, joint_rot_mode='rotmat'``, reference :151-162) and ``root_palm``
-(:248-250) run through ``acr_b200_mano_layer_forward`` / ``_backward`` instead (``_ManoLayerFunction``): the
-SO(3) projection of every input matrix and its gradient are fused into the same kernels.
+(:248-250) run through ``acr_b200_mano_layer_forward`` / ``_backward`` instead: the SO(3) projection of every input
+matrix and its gradient are fused into the same kernels.
+
+Forward mode (``torch.func.jvp`` / ``jacfwd``, ``torch.autograd.forward_ad``) runs the fused JVP kernel
+``acr_b200_mano_layer_jvp``, and every torch.func transform composes with the layer (``vmap``, ``grad``, ``jacrev``):
+the Functions' vmap rules fold a vmapped batch into more hands, or into more tangents / cotangent rows.
 """
 from __future__ import annotations
 
@@ -18,7 +22,7 @@ from typing import Optional
 
 import numpy as np
 import torch
-from torch.autograd.function import once_differentiable
+import torch.autograd.forward_ad as _fwAD
 from torch.nn import Module
 
 from acr_b200 import lib as _lib
@@ -28,58 +32,150 @@ from mano.assets import get_asset
 _ZERO1 = torch.zeros(1)
 
 
+_SECOND_ORDER = ("ManoLayer has first-order derivatives only: double backward and forward-over-reverse "
+                 "(torch.func.hessian, jvp of grad) are not supported")
+
+
+def _batch_first(x, bdim, size):
+    """A vmapped tensor with its batch dim (None: unbatched) moved to the front, of length ``size``."""
+    return x.expand(size, *x.shape) if bdim is None else x.movedim(bdim, 0)
+
+
+def _fold_hands(x, bdim, size, hand_dim=0):
+    """Fold a vmap batch of ``size`` into the hand dimension ``hand_dim``: batch b, hand i -> hand b*n + i.  None
+    (no tensor) passes through."""
+    if x is None:
+        return None
+    x = _batch_first(x, bdim, size).movedim(0, hand_dim)
+    return x.reshape(*x.shape[:hand_dim], -1, *x.shape[hand_dim + 2:])
+
+
+def _unfold_hands(x, size, hand_dim=0):
+    return x.reshape(*x.shape[:hand_dim], size, -1, *x.shape[hand_dim + 1:])
+
+
 class _ManoFunction(torch.autograd.Function):
-    """(pose (n,48) without the mean pose, betas (n,10)) -> (verts, joints, center) of one side; the backward is the
-    fused MANO backward kernel (first order only)."""
+    """(pose: (n,48) axis angles without the mean pose or (n,16,3,3) matrices, betas (n,10)) -> (verts, joints,
+    center) of one side, with ``root_palm``.  Axis angles without the palm run the plain fused forward, the other forms
+    ``acr_b200_mano_layer_forward``.  The backward is the fused backward kernel pair and the JVP the fused JVP kernel,
+    each behind a Function of its own with a vmap rule, so torch.func's transforms compose with them; first order
+    only."""
 
     @staticmethod
-    def forward(ctx, pose, betas, model, side, center_idx):
-        out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose, betas, None, side,
-                                center_idx)
+    def forward(pose, betas, model, side, pose_mode, center_idx, root_palm):
+        if pose_mode == _lib.POSE_AXISANG and not root_palm:
+            out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose, betas, None, side,
+                                    center_idx)
+            return out["verts"], out["joints"], out["center"]
+        return _ops.mano_layer_forward(model, side, pose, pose_mode, betas, center_idx, root_palm)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pose, betas = inputs[:2]
         ctx.save_for_backward(pose, betas)
-        ctx.model, ctx.side, ctx.center_idx = model, side, center_idx
+        ctx.save_for_forward(pose, betas)
+        ctx.args = inputs[2:]
         ctx.set_materialize_grads(False)     # an unused output's cotangent stays None and reaches the kernel as NULL
-        return out["verts"], out["joints"], out["center"]
 
     @staticmethod
-    @once_differentiable
     def backward(ctx, dverts, djoints, dcenter):
         pose, betas = ctx.saved_tensors
-        want_pose, want_betas = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        if ctx.center_idx is None:
+        none = (None,) * 5
+        if ctx.args[3] is None:
             dcenter = None                   # the centre output is zero and does not depend on the inputs
         if dverts is None and djoints is None and dcenter is None:
-            return None, None, None, None, None
-        dpose, dbetas = _ops.mano_backward(ctx.model, ctx.side, pose, betas, ctx.center_idx, dverts, djoints, dcenter,
-                                           want_pose, want_betas)
-        return dpose, dbetas, None, None, None
-
-
-class _ManoLayerFunction(torch.autograd.Function):
-    """(pose: (n,16,3,3) matrices or (n,48) axis angles without the mean pose, betas (n,10)) -> (verts, joints,
-    center) of one side, with ``root_palm``; the backward is the fused kernel pair (first order only)."""
+            return (None, None) + none
+        dpose, dbetas = _ManoVjp.apply(pose, betas, dverts, djoints, dcenter, *ctx.args)
+        return (dpose if ctx.needs_input_grad[0] else None, dbetas if ctx.needs_input_grad[1] else None) + none
 
     @staticmethod
-    def forward(ctx, pose, betas, model, side, pose_mode, center_idx, root_palm):
-        out = _ops.mano_layer_forward(model, side, pose, pose_mode, betas, center_idx, root_palm)
-        ctx.save_for_backward(pose, betas)
-        ctx.args = (model, side, pose_mode, center_idx, root_palm)
-        ctx.set_materialize_grads(False)     # an unused output's cotangent stays None and reaches the kernel as NULL
-        return out
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, dverts, djoints, dcenter):
+    def jvp(ctx, tpose, tbetas, *_):
         pose, betas = ctx.saved_tensors
-        model, side, pose_mode, center_idx, root_palm = ctx.args
-        if center_idx is None:
-            dcenter = None                   # the centre output is zero and does not depend on the inputs
-        none = (None,) * 7
-        if dverts is None and djoints is None and dcenter is None:
-            return none
-        dpose, dbetas = _ops.mano_layer_backward(model, side, pose, pose_mode, betas, center_idx, root_palm, dverts,
-                                                 djoints, dcenter, ctx.needs_input_grad[0], ctx.needs_input_grad[1])
-        return (dpose, dbetas) + none[2:]
+        tv, tj, tc = _ManoJvp.apply(pose, betas, None if tpose is None else tpose.unsqueeze(0),
+                                    None if tbetas is None else tbetas.unsqueeze(0), *ctx.args)
+        return tv[0], tj[0], tc[0]
+
+    @staticmethod
+    def vmap(info, in_dims, pose, betas, *args):
+        # the vmapped dims become more hands
+        B = info.batch_size
+        outs = _ManoFunction.apply(_fold_hands(pose, in_dims[0], B), _fold_hands(betas, in_dims[1], B), *args)
+        return tuple(_unfold_hands(o, B) for o in outs), (0, 0, 0)
+
+
+class _ManoVjp(torch.autograd.Function):
+    """Cotangents of ``_ManoFunction``'s (verts, joints, center) -> (dpose, dbetas): the fused backward kernels."""
+
+    @staticmethod
+    def forward(pose, betas, dverts, djoints, dcenter, model, side, pose_mode, center_idx, root_palm):
+        return _ops.mano_layer_backward(model, side, pose, pose_mode, betas, center_idx, root_palm, dverts, djoints,
+                                        dcenter)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise RuntimeError(_SECOND_ORDER)
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise RuntimeError(_SECOND_ORDER)
+
+    @staticmethod
+    def vmap(info, in_dims, pose, betas, dverts, djoints, dcenter, *args):
+        # a batch of cotangents (jacrev) becomes more rows: pose and betas are repeated for each
+        B = info.batch_size
+        f = [_fold_hands(x, d, B) for x, d in zip((pose, betas, dverts, djoints, dcenter), in_dims)]
+        dpose, dbetas = _ManoVjp.apply(*f, *args)
+        return (_unfold_hands(dpose, B), _unfold_hands(dbetas, B)), (0, 0)
+
+
+class _ManoJvp(torch.autograd.Function):
+    """(pose, betas, tangents tpose (T,n,...) and tbetas (T,n,10), either None) -> the T tangents of
+    ``_ManoFunction``'s outputs, tangent-major: the fused JVP kernel."""
+
+    @staticmethod
+    def forward(pose, betas, tpose, tbetas, model, side, pose_mode, center_idx, root_palm):
+        return _ops.mano_layer_jvp(model, side, pose, pose_mode, betas, center_idx, root_palm, tpose, tbetas)
+
+    @staticmethod
+    def setup_context(ctx, inputs, output):
+        pass
+
+    @staticmethod
+    def backward(ctx, *grads):
+        raise RuntimeError(_SECOND_ORDER)
+
+    @staticmethod
+    def jvp(ctx, *tangents):
+        raise RuntimeError(_SECOND_ORDER)
+
+    @staticmethod
+    def vmap(info, in_dims, pose, betas, tpose, tbetas, *args):
+        B = info.batch_size
+        if in_dims[0] is None and in_dims[1] is None:
+            # only the tangents are batched (jacfwd): they become more tangents of the same hands, one launch
+            f = [None if x is None else _batch_first(x, d, B).flatten(0, 1) for x, d in ((tpose, in_dims[2]),
+                                                                                        (tbetas, in_dims[3]))]
+            outs = _ManoJvp.apply(pose, betas, *f, *args)
+            return tuple(o.unflatten(0, (B, -1)) for o in outs), (0, 0, 0)
+        # the hands are batched: the batch becomes more hands, each with its own tangents
+        outs = _ManoJvp.apply(_fold_hands(pose, in_dims[0], B), _fold_hands(betas, in_dims[1], B),
+                              _fold_hands(tpose, in_dims[2], B, 1), _fold_hands(tbetas, in_dims[3], B, 1), *args)
+        return tuple(_unfold_hands(o, B, 1) for o in outs), (1, 1, 1)
+
+
+def _differentiated(*ts) -> bool:
+    """Whether the forward must run inside ``_ManoFunction``: autograd will differentiate it, a torch.func transform
+    is active (its wrapped tensors cannot go to the kernels directly), or an input is a forward-AD dual tensor.
+    Otherwise the forward makes the plain launch."""
+    if torch._C._are_functorch_transforms_active():
+        return True
+    if torch.is_grad_enabled() and any(t.requires_grad for t in ts):
+        return True
+    return _fwAD._current_level >= 0 and any(_fwAD.unpack_dual(t).tangent is not None for t in ts)
 
 
 def _rodrigues(aa: torch.Tensor) -> torch.Tensor:
@@ -147,13 +243,15 @@ class ManoLayer(Module):
             (() if hm is None else (hm,))
         key = tuple((b._version, b.data_ptr(), str(b.device)) for b in bufs)
         if self._packed is None or key != self._packed_key:
-            asset = dict(shapedirs=self.th_shapedirs.detach().cpu().numpy(),
-                         posedirs=self.th_posedirs.detach().cpu().numpy(),
-                         v_template=self.th_v_template[0].detach().cpu().numpy(),
-                         J_regressor=self.th_J_regressor.detach().cpu().numpy(),
-                         weights=self.th_weights.detach().cpu().numpy(),
-                         hands_mean=np.zeros(45, np.float32) if hm is None else hm[0].detach().cpu().numpy())
-            self._packed = _ops.pack_mano_model(asset, False, self.th_shapedirs.device)
+            # the buffers are constants: read them as such also when the first call runs inside a torch.func transform
+            with torch._C._DisableFuncTorch():
+                asset = dict(shapedirs=self.th_shapedirs.detach().cpu().numpy(),
+                             posedirs=self.th_posedirs.detach().cpu().numpy(),
+                             v_template=self.th_v_template[0].detach().cpu().numpy(),
+                             J_regressor=self.th_J_regressor.detach().cpu().numpy(),
+                             weights=self.th_weights.detach().cpu().numpy(),
+                             hands_mean=np.zeros(45, np.float32) if hm is None else hm[0].detach().cpu().numpy())
+                self._packed = _ops.pack_mano_model(asset, False, self.th_shapedirs.device)
             self._packed_key = key
         return self._packed
 
@@ -183,15 +281,12 @@ class ManoLayer(Module):
             raise NotImplementedError("centring on the palm (center_idx=0 with root_palm) is not supported")
         side = 1 if self.side == 'right' else 0
         model = self.packed_model()
-        if self.rotmat or palm:
-            mode = _lib.POSE_ROTMAT if self.rotmat else _lib.POSE_AXISANG
-            p = pose if self.rotmat else pose[:, :48]
-            if torch.is_grad_enabled() and (p.requires_grad or betas.requires_grad):
-                verts, jtr, center = _ManoLayerFunction.apply(p, betas, model, side, mode, center_idx, palm)
-            else:
-                verts, jtr, center = _ops.mano_layer_forward(model, side, p, mode, betas, center_idx, palm)
-        elif torch.is_grad_enabled() and (pose.requires_grad or betas.requires_grad):
-            verts, jtr, center = _ManoFunction.apply(pose[:, :48], betas, model, side, center_idx)
+        mode = _lib.POSE_ROTMAT if self.rotmat else _lib.POSE_AXISANG
+        p = pose if self.rotmat else pose[:, :48]
+        if _differentiated(p, betas):
+            verts, jtr, center = _ManoFunction.apply(p, betas, model, side, mode, center_idx, palm)
+        elif self.rotmat or palm:
+            verts, jtr, center = _ops.mano_layer_forward(model, side, p, mode, betas, center_idx, palm)
         else:
             out = _ops.mano_forward(model if side == 0 else None, model if side == 1 else None, pose[:, :48],
                                     betas, None, side, center_idx)

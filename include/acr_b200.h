@@ -150,6 +150,22 @@ int acr_b200_mano_layer_backward(const float* model, int side, const float* pose
                                  const float* djoints, const float* dcenter, float* workspace, float* dpose,
                                  float* dbetas, void* stream);
 
+/* Forward-mode derivative (Jacobian-vector products) of acr_b200_mano_layer_forward, n_tan tangents per hand.
+ *   model ... root_palm : as in acr_b200_mano_layer_forward (the same ACR_B200_ENOTSUP / EINVAL cases).
+ *   tpose  : (n_tan, n, 48) or (n_tan, n, 16, 3, 3), tangents of pose; tbetas (n_tan, n, 10).  NULL = zero.
+ *   verts, joints, center : the primal outputs, as in the forward; any may be NULL.
+ *   tverts (n_tan, n, 778, 3), tjoints (n_tan, n, 21, 3), tcenter (n_tan, n, 3) : the output tangents, tangent-major;
+ *            any may be NULL.  tcenter is zero without a centre.
+ * In rotation-matrix mode the projection's tangent is the polar factor's, finite at exact rotations; at a zero axis
+ * angle the Rodrigues tangent is finite too.  With verts and tverts both NULL only the 16 joints, the tips and the
+ * palm are computed (one CTA per 8 hands and 4 tangents): a keypoint Jacobian costs no vertex pass.  fp32, no
+ * atomics; a tangent's result does not depend on n_tan or on the other tangents, and repeated calls are
+ * bit-identical.  n_tan < 0 is ACR_B200_EINVAL.                                                                */
+int acr_b200_mano_layer_jvp(const float* model, int side, const float* pose, int pose_mode, const float* betas, int n,
+                            int center_idx, int root_palm, int n_tan, const float* tpose, const float* tbetas,
+                            float* verts, float* joints, float* center, float* tverts, float* tjoints, float* tcenter,
+                            void* stream);
+
 /* Camera translation of every hand from its 21 joints: the closed-form weighted least squares of
  * estimate_translation_np (acr/utils.py:430-472) -- the reference's own fall-back for the host-side
  * cv2.solvePnPRansac loop (estimate_translation :474-519, called from vertices_kp3d_projection :403-407,
