@@ -18,7 +18,9 @@ _DEFAULTS = dict(
                                                           # values starting with "resnet" select the ResNet-50 trunk
                                                           # (backbone_kind), every other value the HRNet trunk
     model_precision="bf16",                               # reference: fp32|fp16 (config.py:96); here bf16|fp16 = tensor-core
-                                                          # plans, fp32 = the (slow, reference-accurate) validation plan
+                                                          # plans, fp32 = the (slow, reference-accurate) validation plan,
+                                                          # tf32 = fp32 storage with tf32 tensor-core convs (what the
+                                                          # reference's fp32 runs as on Ampere / Hopper with cuDNN's TF32)
     hrnet_width=32,                                        # 32 = the reference's HRNet-W32 (the only trunk it contains); 48 = the
                                                           # HRNet-W48 trunk of BASELINE configs[4] (no reference: parity unpinned)
     input_size=512,                                        # config.py:61

@@ -98,8 +98,8 @@ class ACR(nn.Module):
             _attach(self, key, t, is_param=kind not in ('bn_mean', 'bn_var', 'bn_nbt'))
         self._result_parser = ResultParser()
         self.outmap_size = args().centermap_size
-        self._engines = OrderedDict()     # LRU of launch plans, keyed by (batch, device, dtype, flags, heads-only)
-        self._blobs = {}                  # packed weights, shared by every plan of one (device, dtype, flags)
+        self._engines = OrderedDict()     # LRU of launch plans, keyed by (batch, device, dtype, tf32, flags, heads-only)
+        self._blobs = {}                  # packed weights, shared by every plan of one (device, dtype, tf32, flags)
         self.max_engines = int(kwargs.get('max_engines', 3))
         self.debug_ref_conv = bool(kwargs.get('debug_ref_conv', False))
 
@@ -119,36 +119,45 @@ class ACR(nn.Module):
         """'bf16' / 'fp16': 16-bit storage, fp32 accumulation on the tensor cores (fp16 is the reference's
         autocast mode, acr/model.py:36-41).  'fp32' (the reference's shipped default, configs/demo.yml:7):
         the validation plan -- fp32 storage, fp64 accumulation on the CUDA cores -- reference-accurate
-        (1e-4 end to end) but ~100x slower than the 16-bit plans."""
+        (1e-4 end to end) but ~100x slower than the 16-bit plans.  'tf32': fp32 storage and outputs with every conv
+        but the stem on the tensor cores with tf32 operands -- what the reference's fp32 model runs as on Ampere /
+        Hopper, where cuDNN convolutions default to TF32 (the TF32 plan; ``_tf32`` tells it from 'fp32')."""
         p = args().model_precision
         if p == 'bf16':
             return torch.bfloat16
         if p == 'fp16':
             return torch.float16
+        if p == 'tf32':
+            return torch.float32
         if p == 'fp32':
             if not ACR._warned_fp32:
                 logging.warning("model_precision='fp32' runs the fp32 validation plan on the CUDA cores (reference-"
                                 "accurate, slow); use 'fp16' (the reference's autocast mode) or 'bf16' for throughput")
                 ACR._warned_fp32 = True
             return torch.float32
-        raise ValueError(f"model_precision must be 'fp32', 'fp16' or 'bf16', got {p!r}")
+        raise ValueError(f"model_precision must be 'fp32', 'tf32', 'fp16' or 'bf16', got {p!r}")
+
+    @staticmethod
+    def _tf32():
+        return args().model_precision == 'tf32'
 
     def engine(self, batch: int, device, head_only: bool = False) -> Engine:
         """Launch plan for this batch size (built on first use).  Plans share one packed weight blob per
-        (device, dtype); at most ``max_engines`` plans (each owns a ~26 MiB/image activation arena) are kept,
+        (device, dtype, TF32 or not); at most ``max_engines`` plans (each owns a ~26 MiB/image activation arena) are kept,
         least recently used first out -- variable batch sizes (the last partial batch of a video) do not
         accumulate GPU memory."""
-        dt = self._act_dtype()
+        dt, tf32 = self._act_dtype(), self._tf32()
         dev = torch.device(device)
         if dev.type == 'cuda' and dev.index is None:
             dev = torch.device('cuda', torch.cuda.current_device())
-        bkey = (str(dev), dt, self.debug_ref_conv, head_only)
+        bkey = (str(dev), dt, tf32, self.debug_ref_conv, head_only)   # 'tf32' and 'fp32' plans share no weights
         key = (batch,) + bkey
         if key in self._engines:
             self._engines.move_to_end(key)
             return self._engines[key]
         eng = Engine(self.state_dict(), batch, dev, dt, args().input_size, debug_ref_conv=self.debug_ref_conv,
-                     head_only=head_only, weights=self._blobs.get(bkey), widths=self._widths, backbone=self._backbone)
+                     head_only=head_only, weights=self._blobs.get(bkey), widths=self._widths, backbone=self._backbone,
+                     tf32=tf32)
         self._blobs[bkey] = eng.weights
         self._engines[key] = eng
         while len(self._engines) > max(1, self.max_engines):

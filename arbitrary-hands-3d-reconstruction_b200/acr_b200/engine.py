@@ -107,6 +107,10 @@ class Engine:
     product path on the tensor cores -- or torch.float32: the VALIDATION plan (fp32 storage, fp64
     accumulation on the CUDA cores, csrc/validate_f32.cu), which is what the reference's default
     ``model_precision='fp32'`` maps to and what pins the whole pipeline at 1e-4.
+    ``tf32=True`` (with act_dtype torch.float32): the TF32 plan, ``model_precision='tf32'`` -- what the reference's fp32
+    model runs on Ampere / Hopper under cuDNN's default ``allow_tf32``.  The validation plan's op list and arena (fp32
+    storage, no x-pair / stride-2 pair packing, no fused blocks, CUDA-core stem), but every conv on the wgmma tensor cores
+    with tf32 operands and fp32 accumulation, its weights packed as DT_TF32 (BN folded, rounded to the nearest tf32).
     ``debug_ref_conv`` swaps the wgmma conv for the CUDA-core reference kernel (tests only).
     ``head_only`` builds the plan of ``ACR.head_forward`` (/root/reference/acr/model.py:47-65): the ops
     after the trunk, fed by an external (B,32,H/4,W/4) feature through ``run_heads``.
@@ -114,14 +118,14 @@ class Engine:
     not depend on the batch size).
     ``backbone``: "hrnet" (HRNet-W32, or the trunk ``widths`` names) or "resnet50" (netspec.build_acr_spec): the
     ResNet-50 trunk runs on the tensor cores only (7x7 stem, max-pool, 1x1 stride-2 and transposed convs have no fp32
-    validation or CUDA-core form), so fp32 and ``debug_ref_conv`` raise AcrB200Error for it.
+    validation or CUDA-core form), so fp32, ``tf32`` and ``debug_ref_conv`` raise AcrB200Error for it.
     """
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], batch: int, device, act_dtype=torch.bfloat16,
                  input_size: int = 512, debug_ref_conv: bool = False, reuse_memory: bool = True,
                  dry_run: bool = False, keep_extra=(), stem_on_tensor_cores: bool = True,
                  head_only: bool = False, weights: Optional[torch.Tensor] = None, widths=None,
-                 backbone: str = "hrnet"):
+                 backbone: str = "hrnet", tf32: bool = False):
         self.keep_extra = tuple(keep_extra)   # extra tensor names kept alive after the run (tests)
         self.dry_run = dry_run      # layout only (arena size, op list); used by CPU tests
         if not dry_run and not torch.cuda.is_available():
@@ -134,11 +138,15 @@ class Engine:
         self.act_dtype = act_dtype
         self.dt = {torch.bfloat16: L.DT_BF16, torch.float16: L.DT_F16, torch.float32: L.DT_F32}[act_dtype]
         self.f32 = act_dtype == torch.float32
+        if tf32 and not self.f32:
+            raise L.AcrB200Error("Engine: tf32=True is the TF32 plan of fp32 storage: pass act_dtype=torch.float32")
+        self.tf32 = bool(tf32)
+        self.plan_dt = L.DT_TF32 if self.tf32 else self.dt   # act_dtype of the plan and the weight packer
         self.esz = 4 if self.f32 else 2
         self.npw = np.float32 if self.f32 else np.uint16      # numpy type of one packed weight
         if backbone == "resnet50" and (self.f32 or debug_ref_conv):
-            raise L.AcrB200Error("Engine: the ResNet-50 trunk runs on the tensor cores only (no fp32 validation plan, "
-                                 "no debug_ref_conv): use act_dtype torch.bfloat16 or torch.float16")
+            raise L.AcrB200Error("Engine: the ResNet-50 trunk runs on the tensor cores only (no fp32 validation or TF32 "
+                                 "plan, no debug_ref_conv): use act_dtype torch.bfloat16 or torch.float16")
         self.backbone = backbone
         self.stem_on_tensor_cores = stem_on_tensor_cores and not self.f32
         self.head_only = head_only
@@ -152,7 +160,7 @@ class Engine:
                                             backbone=backbone)
         self.input_size = input_size
         self.flops_per_image = conv_flops_per_image(self.spec)
-        self.debug_ref_conv = debug_ref_conv or self.f32
+        self.debug_ref_conv = debug_ref_conv or (self.f32 and not self.tf32)
         self.run_count = 0          # bumped by every run(): lazily read outputs check it (acr/model.py)
         sd = {k: v.detach().float().cpu().numpy() for k, v in (state_dict or {}).items()
               if v.dtype.is_floating_point}
@@ -193,7 +201,7 @@ class Engine:
         bias = np.zeros(cout_pad, np.float32)
         p = lambda a: None if a is None else a.ctypes.data
         L.check(self.lib.acr_b200_pack_conv(p(w), p(cb), p(bn[0]), p(bn[1]), p(bn[2]), p(bn[3]), BN_EPS, cout, cin, k,
-                                            cout_pad, cin_pad, self.dt, wp.ctypes.data, bias.ctypes.data),
+                                            cout_pad, cin_pad, self.plan_dt, wp.ctypes.data, bias.ctypes.data),
                 "pack_conv " + wkey)
         return blob.add(wp), blob.add(bias)
 
@@ -208,7 +216,7 @@ class Engine:
         for p in range(4):
             w = np.ascontiguousarray(par[p])
             L.check(self.lib.acr_b200_pack_conv(w.ctypes.data, None, *(b.ctypes.data for b in bn), BN_EPS, cout, cin, 2,
-                                                cout_pad, cin_pad, self.dt, wp[p].ctypes.data, bias.ctypes.data),
+                                                cout_pad, cin_pad, self.plan_dt, wp[p].ctypes.data, bias.ctypes.data),
                     "pack_conv " + wkey)
         return blob.add(wp), blob.add(bias)
 
@@ -218,7 +226,7 @@ class Engine:
         bias = np.zeros(cout_pad, np.float32)
         w = np.ascontiguousarray(w, np.float32)
         L.check(self.lib.acr_b200_pack_conv(w.ctypes.data, None, None, None, None, None, BN_EPS, cout, cin, k,
-                                            cout_pad, cin_pad, self.dt, wp.ctypes.data, bias.ctypes.data), "pack_conv")
+                                            cout_pad, cin_pad, self.plan_dt, wp.ctypes.data, bias.ctypes.data), "pack_conv")
         return blob.add(wp)
 
     # --------------------------------------------------------------------- plan
@@ -523,7 +531,7 @@ class Engine:
             self.arena = torch.zeros(self.arena_bytes, dtype=torch.uint8, device=self.device)
             plan = C.c_void_p()
             L.check(self.lib.acr_b200_plan_create(cops, len(recs), B, self.arena.data_ptr(), self.arena_bytes,
-                                                  self.weights.data_ptr(), self.weights.numel(), self.dt, C.byref(plan)),
+                                                  self.weights.data_ptr(), self.weights.numel(), self.plan_dt, C.byref(plan)),
                     "plan_create")
         self.plan = plan
 

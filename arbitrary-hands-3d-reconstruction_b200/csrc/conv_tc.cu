@@ -35,7 +35,9 @@ static int encode(CUtensorMap* m, int act_dtype, int rank, const void* ptr, cons
   if (!fn) { set_error("conv_tc: cuTensorMapEncodeTiled unavailable (no CUDA driver?)"); return ACR_B200_ECUDA; }
   cuuint32_t es[5] = {1, 1, 1, 1, 1};
   const CUtensorMapSwizzle sw = ck == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (ck == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
-  const CUtensorMapDataType dt = act_dtype == ACR_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  // (TF32 plan: fp32 tensors are described as 16-bit words, two per channel; see conv_tc_prepare)
+  const CUtensorMapDataType dt = act_dtype == ACR_DT_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : (act_dtype == ACR_DT_TF32 ? CU_TENSOR_MAP_DATA_TYPE_UINT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
   CUresult r = fn(m, dt, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("conv_tc: cuTensorMapEncodeTiled failed (%d)", (int)r); return ACR_B200_ECUDA; }
@@ -61,7 +63,16 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   ACR_CHECK_ARG(a.out.H % TILE_Y == 0 && a.out.W % TILE_X == 0, "conv_tc: output %dx%d is not a multiple of the 16x16 super-tile", a.out.H, a.out.W);
   ACR_CHECK_ARG(a.in.pix_stride % 8 == 0 && a.cin_pad % 16 == 0 && a.cout_pad % 16 == 0 && a.cout_pad <= 2048 && a.cin_pad <= 2048,
                 "conv_tc: channel alignment");
-  ACR_CHECK_ARG(a.in.dtype == act_dtype, "conv_tc: input dtype mismatch");
+  // TF32 plan (act_dtype ACR_DT_TF32): fp32 tensors and weights, described to the TMA unit as 16-bit words, two per
+  // channel -- byte-identical, for boxes, swizzle and descriptors, to a 16-bit tensor of twice the channels.  So every
+  // channel count, chunk (ck) and stride below is in 16-bit units: ck = 64 / 32 holds 32 / 16 fp32 channels.
+  const bool tf32 = act_dtype == ACR_DT_TF32;
+  const int ew = tf32 ? 2 : 1;   // 16-bit words per element
+  ACR_CHECK_ARG(a.in.dtype == (tf32 ? ACR_DT_F32 : act_dtype), "conv_tc: input dtype mismatch");
+  ACR_CHECK_ARG(!tf32 || (a.out.dtype == ACR_DT_F32 && (!a.has_res || a.res.dtype == ACR_DT_F32) && !a.xpair && !a.s2x &&
+                          !a.deconv && a.n_ext == 0),
+                "conv_tc: the tf32 conv reads and writes fp32 tensors and has no x-paired, transposed or extra-term form");
+  const int cin_pad = a.cin_pad * ew, in_stride = a.in.pix_stride * ew;
   ACR_CHECK_ARG(!a.deconv || (a.k == 4 && a.stride == 2 && a.cin_pad % 64 == 0 && !a.has_res && a.n_ext == 0 && !a.xpair &&
                               !a.s2x && !a.bias_per_image && !a.pow11_ch0 && a.out.H == 2 * a.in.H && a.out.W == 2 * a.in.W &&
                               a.in.H % TILE_Y == 0 && a.in.W % TILE_X == 0),
@@ -73,7 +84,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
                            a.in.H == 2 * a.out.H && a.in.W == a.out.W),
                 "conv_tc: the x-paired stride-2 form reads a dense 32-channel tensor as (H, W/2, 64)");
   ACR_CHECK_ARG(a.out.pix_stride % 2 == 0 && (!a.has_res || a.res.pix_stride % 2 == 0), "conv_tc: output / residual rows must hold channel pairs");
-  const int ck = (a.cin_pad % 64 == 0) ? 64 : ((a.cin_pad % 32 == 0) ? 32 : 16);
+  const int ck = (cin_pad % 64 == 0) ? 64 : ((cin_pad % 32 == 0) ? 32 : 16);
   ConvTcPlan* pl = new ConvTcPlan();
   ConvTcParams& p = pl->p;
   pl->ck = ck; pl->act_dtype = act_dtype;
@@ -86,22 +97,22 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   const cuuint32_t box_rows = p.s2x ? TILE_Y + 1 : ((p.patch_mode || p.deconv) ? TILE_Y + 2 : TILE_Y);
   const cuuint32_t box_cols = (p.patch1 || p.s2x || p.deconv) ? P1_PITCH : TILE_X;
   const cuuint64_t esz = 2;
-  const cuuint64_t dim0 = (cuuint64_t)(a.cin_pad < a.in.pix_stride ? a.cin_pad : a.in.pix_stride);
+  const cuuint64_t dim0 = (cuuint64_t)(cin_pad < in_stride ? cin_pad : in_stride);
   int rc = ACR_B200_OK;
   if (a.s2x) {   // two row-parity views of the x-paired input (H, W/2, 64): rows 2r + py
     for (int v = 0; v < 2 && !rc; ++v) {
-      const char* ptr = static_cast<const char*>(a.in.ptr) + (size_t)v * a.in.W * a.in.pix_stride * esz;
+      const char* ptr = static_cast<const char*>(a.in.ptr) + (size_t)v * a.in.W * in_stride * esz;
       cuuint64_t dims[4] = {dim0, (cuuint64_t)a.in.W, (cuuint64_t)a.in.H / 2, (cuuint64_t)a.batch};
-      cuuint64_t str[3] = {(cuuint64_t)a.in.pix_stride * esz, (cuuint64_t)2 * a.in.W * a.in.pix_stride * esz,
-                           (cuuint64_t)a.in.H * a.in.W * a.in.pix_stride * esz};
+      cuuint64_t str[3] = {(cuuint64_t)in_stride * esz, (cuuint64_t)2 * a.in.W * in_stride * esz,
+                           (cuuint64_t)a.in.H * a.in.W * in_stride * esz};
       cuuint32_t box[4] = {(cuuint32_t)ck, box_cols, box_rows, 1};
       rc = encode(&p.tmA[v], act_dtype, 4, ptr, dims, str, box, ck);
     }
     for (int v = 2; v < 4 && !rc; ++v) p.tmA[v] = p.tmA[0];
   } else if (a.stride == 1 || a.deconv) {   // (the transposed conv reads its input at stride 1)
     cuuint64_t dims[4] = {dim0, (cuuint64_t)a.in.W, (cuuint64_t)a.in.H, (cuuint64_t)a.batch};
-    cuuint64_t str[3] = {(cuuint64_t)a.in.pix_stride * esz, (cuuint64_t)a.in.W * a.in.pix_stride * esz,
-                         (cuuint64_t)a.in.H * a.in.W * a.in.pix_stride * esz};
+    cuuint64_t str[3] = {(cuuint64_t)in_stride * esz, (cuuint64_t)a.in.W * in_stride * esz,
+                         (cuuint64_t)a.in.H * a.in.W * in_stride * esz};
     cuuint32_t box[4] = {(cuuint32_t)ck, box_cols, box_rows, 1};
     rc = encode(&p.tmA[0], act_dtype, 4, a.in.ptr, dims, str, box, ck);
     for (int v = 1; v < 4 && !rc; ++v) p.tmA[v] = p.tmA[0];
@@ -109,10 +120,10 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
     // four parity views (even / odd rows x columns); a 1x1 stride-2 conv (padding 0) reads view 0 at offset 0 only
     for (int v = 0; v < 4 && !rc; ++v) {
       const int py = v >> 1, px = v & 1;
-      const char* ptr = static_cast<const char*>(a.in.ptr) + ((size_t)py * a.in.W + px) * a.in.pix_stride * esz;
+      const char* ptr = static_cast<const char*>(a.in.ptr) + ((size_t)py * a.in.W + px) * in_stride * esz;
       cuuint64_t dims[4] = {dim0, (cuuint64_t)a.in.W / 2, (cuuint64_t)a.in.H / 2, (cuuint64_t)a.batch};
-      cuuint64_t str[3] = {(cuuint64_t)2 * a.in.pix_stride * esz, (cuuint64_t)2 * a.in.W * a.in.pix_stride * esz,
-                           (cuuint64_t)a.in.H * a.in.W * a.in.pix_stride * esz};
+      cuuint64_t str[3] = {(cuuint64_t)2 * in_stride * esz, (cuuint64_t)2 * a.in.W * in_stride * esz,
+                           (cuuint64_t)a.in.H * a.in.W * in_stride * esz};
       cuuint32_t box[4] = {(cuuint32_t)ck, TILE_X, box_rows, 1};
       rc = encode(&p.tmA[v], act_dtype, 4, ptr, dims, str, box, ck);
     }
@@ -141,7 +152,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   }
   p.stage_out_bytes = p.tma_out ? 4u * 8192u : 0u;
   p.bias = a.bias; p.res = a.has_res ? a.res.ptr : nullptr; p.out = a.out.ptr;
-  p.taps = a.deconv ? 4 : a.k * a.k; p.ksz = a.k; p.stride = a.stride; p.cchunks = a.cin_pad / ck; p.cin_pad = a.cin_pad;
+  p.taps = a.deconv ? 4 : a.k * a.k; p.ksz = a.k; p.stride = a.stride; p.cchunks = cin_pad / ck; p.cin_pad = cin_pad;
   p.npad = a.cout_pad; p.nsplit = nsplit; p.nsub = nsub;
   pl->nt = nsub <= 64 ? 64 : 128;   // MMA width (a compile-time kernel parameter): the columns past nsub are not stored
   p.relu = a.relu; p.has_res = a.has_res; p.out_f32 = a.out.dtype == ACR_DT_F32;
@@ -168,8 +179,8 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   p.b_block_bytes = (uint32_t)(p.b_resident ? a.cout_pad : pl->nt) * ck * 2;
   {
     const int taps = p.taps;
-    cuuint64_t dims[2] = {(cuuint64_t)taps * a.cin_pad, (cuuint64_t)npar * a.cout_pad};
-    cuuint64_t str[1] = {(cuuint64_t)taps * a.cin_pad * esz};
+    cuuint64_t dims[2] = {(cuuint64_t)taps * cin_pad, (cuuint64_t)npar * a.cout_pad};
+    cuuint64_t str[1] = {(cuuint64_t)taps * cin_pad * esz};
     cuuint32_t box[2] = {(cuuint32_t)ck, (cuuint32_t)(p.b_resident ? a.cout_pad : pl->nt)};   // rows past cout_pad: zero fill
     rc = encode(&p.tmB, act_dtype, 2, a.w, dims, str, box, ck);
     if (rc) { delete pl; return rc; }
@@ -202,6 +213,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
 }
 
 int conv_tc_launch(const ConvTcPlan* pl, cudaStream_t st) {
+  if (pl->act_dtype == ACR_DT_TF32) return conv_tc_launch_tf32(pl, st);
   const bool bf = pl->act_dtype == ACR_DT_BF16;
   switch (pl->ck) {
     case 64: return bf ? conv_tc_launch_64_bf16(pl, st) : conv_tc_launch_64_f16(pl, st);

@@ -29,6 +29,12 @@
 //     gives registers to the consumers (setmaxnreg).
 //   * Resident weights: the consumers run as two ping-pong teams by row group (warpgroups {0,1} and {2,3}), so one team's
 //     epilogue overlaps the other team's MMAs.  Streamed weights: all four warpgroups issue in lockstep.
+//   * T = float (the TF32 plan): fp32 activations and weights, tf32 MMAs with fp32 accumulation.  All shared-memory geometry
+//     is in bytes, and CK counts 16-bit channels: an fp32 NHWC tensor with C channels is, for the TMA boxes, the swizzle
+//     and the descriptors, byte-identical to a 16-bit tensor with 2C channels (CK = 64 / 32 hold 32 / 16 fp32 channels),
+//     and one k8 tf32 step reads the 32 bytes of K of one k16 16-bit step.  The three otherwise idle producer warps round
+//     every landed A stage to the nearest tf32 before the consumers read it (readyA).  The residual is read and the output
+//     stored as fp32.  No x-paired, x-paired stride-2 or transposed form, no extra terms, no TMA-store epilogue.
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -208,6 +214,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   static_assert(!S2X || (!PATCH && !P1 && !XPAIR && CK == 64), "the x-paired stride-2 form is a CK = 64 mode of its own");
   static_assert(!DECONV || (MODE == MODE_DECONV && CK == 64), "the transposed conv is a CK = 64 streamed-weight mode of its own");
   static_assert((NT == 64 || NT == 128) && (!XPAIR || NT == 64), "MMA width: 64 or 128 columns (x-paired convs: 64)");
+  // a 32-channel fp32 pixel already fills a 128-byte row: nothing to pair, and stride-2 convs read the four parity views
+  static_assert(!IsF32<T>::value || !(XPAIR || S2X || DECONV), "fp32 (tf32) operands: no x-paired, stride-2 x-paired or transposed form");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;  // swizzle atoms need 1024-byte alignment
@@ -224,6 +232,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   auto emptyB = [&](int s) { return bar_base + 8u * (2 * SA + SB + s); };
   const uint32_t bres_bar = bar_base + 8u * (2 * SA + 2 * SB);
   const uint32_t dummy_bar = bres_bar + 8u;   // target of the "no stage" arrivals of the consumers (never waited on)
+  // T = float: readyA[SA] after the dummy -- stage s rounded to tf32 (see the producer); the consumers wait on it instead
+  // of fullA
+  auto readyA = [&](int s) { return dummy_bar + 8u * (1 + s); };
+  auto stageA = [&](int s) {
+    if constexpr (IsF32<T>::value) return readyA(s);
+    else return fullA(s);
+  };
   float* s_bias = reinterpret_cast<float*>(smem_raw + (bias_base - raw));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -236,6 +251,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     for (int s = 0; s < SB; ++s) { mbar_init(fullB(s), 1); mbar_init(emptyB(s), CONSUMER_WARPS); }
     mbar_init(bres_bar, 1);
     mbar_init(dummy_bar, 1);
+    if constexpr (IsF32<T>::value)
+      for (int s = 0; s < SA; ++s) mbar_init(readyA(s), 3);
     fence_barrier_init();
     tma_prefetch_desc(&P.tmB);
     tma_prefetch_desc(&P.tmA[0]);
@@ -252,6 +269,38 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     // ===================================================================== TMA producer warpgroup
     // (one warp issues: it stays converged and one elected lane issues; the other three only give up registers)
     setmaxnreg_dec<PRODUCER_REGS>();
+    if constexpr (IsF32<T>::value) {
+      if (warp != PRODUCER_WARP) {
+        // the other three warps: once a stage has landed, round its fp32 activations in place to the nearest tf32
+        // (cvt.rna: ties away from zero), make the writes visible to the MMAs (async proxy) and release the stage to the
+        // consumers.  Fed as stored, the tensor cores would drop the low 13 bits of every activation: a bias of half a
+        // tf32 ulp per product, which the network accumulates (DESIGN.md, TF32 plan).  The weights are rounded on the host.
+        const int ct = threadIdx.x - 32 * (PRODUCER_WARP + 1);
+        int sa = 0;
+        uint32_t pha = 0;
+        for (int vt = blockIdx.x; vt < P.total_tiles * P.nsplit; vt += gridDim.x)
+          for (int a = 0; a < nA; ++a) {
+            mbar_wait_parity(fullA(sa), pha);
+            {
+              uint4* st = reinterpret_cast<uint4*>(smem_raw + (a_base - raw) + (uint32_t)sa * P.a_stage_bytes);
+              for (uint32_t i = ct; i < P.a_stage_bytes / 16u; i += 96) {
+                const float4 v = reinterpret_cast<const float4*>(st)[i];
+                uint4 r;
+                asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r.x) : "f"(v.x));
+                asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r.y) : "f"(v.y));
+                asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r.z) : "f"(v.z));
+                asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r.w) : "f"(v.w));
+                st[i] = r;
+              }
+              fence_proxy_async();
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(readyA(sa));
+            if (++sa == SA) { sa = 0; pha ^= 1u; }
+          }
+        return;
+      }
+    }
     if (warp != PRODUCER_WARP) return;
     if (P.b_resident && elect_one_sync()) {  // whole weight tensor once per CTA
       const int nblk = P.taps * P.cchunks;
@@ -355,7 +404,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   const uint32_t b_lo_base0 = ((b_base >> 4) & 0x3FFF) | lo_flags;
   const uint32_t b_block16 = P.b_block_bytes >> 4, a_stage16 = P.a_stage_bytes >> 4;
   const int cchunks = P.cchunks, taps = P.taps, nsub = P.nsub;
-  const bool tma_out = P.tma_out != 0;
+  const bool tma_out = P.tma_out != 0;   // (16-bit outputs only: conv_tc_prepare)
   const int wg_thread = threadIdx.x & 127;
   const uint32_t stage_wg = stage_base + (uint32_t)wg * 8192u;      // this warpgroup's output slab (TMA-store epilogue)
   const uint32_t is_lane0 = lane == 0 ? 1u : 0u;
@@ -413,7 +462,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       const int par = (vt / P.nsplit) & 3;
       const uint32_t a_par = a_lo_base + (uint32_t)(par >> 1) * pitch16 + (uint32_t)(par & 1) * (Cfg::kRowBytes >> 4);
       for (int cc = 0; cc < cchunks; ++cc) {
-        mbar_wait_parity(fullA(sa), pha);
+        mbar_wait_parity(stageA(sa), pha);
         const uint32_t a_lo = a_par + (uint32_t)sa * a_stage16;
 #pragma unroll
         for (int t = 0; t < 4; ++t) {
@@ -430,7 +479,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       // (kx != 0), K half (kx != 1) -> k-steps {0,1} or {2,3} of the 64-wide row, same k-steps of the weight block
 #pragma unroll
       for (int v = 0; v < 2; ++v) {
-        mbar_wait_parity(fullA(sa), pha);
+        mbar_wait_parity(stageA(sa), pha);
         const uint32_t a_lo = a_lo_base + (uint32_t)sa * a_stage16;
         if (RESIDENT) wgmma_fence();
 #pragma unroll
@@ -456,7 +505,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     } else if (P1) {
       // one A stage per channel chunk; tap (ky,kx) starts (ky * 24 + kx) pixels into it
       for (int cc = 0; cc < cchunks; ++cc) {
-        mbar_wait_parity(fullA(sa), pha);
+        mbar_wait_parity(stageA(sa), pha);
         const uint32_t a_lo = a_lo_base + (uint32_t)sa * a_stage16;
         if (RESIDENT) wgmma_fence();
 #pragma unroll
@@ -482,7 +531,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       uint32_t a_lo[3];
 #pragma unroll
       for (int i = 0; i < 3; ++i) {   // box i holds kx = patch_kx(i) = 1, 0, 2
-        mbar_wait_parity(fullA(sa), pha);
+        mbar_wait_parity(stageA(sa), pha);
         a_lo[i] = a_lo_base + (uint32_t)sa * a_stage16;
         xa_bar[i] = emptyA(sa);
         if (++sa == SA) { sa = 0; pha ^= 1u; }
@@ -502,7 +551,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
           const int kx = XPAIR ? (i == 0 ? 1 : (i == 1 ? 0 : 2)) : i;
-          mbar_wait_parity(fullA(sa), pha);
+          mbar_wait_parity(stageA(sa), pha);
           const uint32_t a_lo = a_lo_base + (uint32_t)sa * a_stage16;
           if (RESIDENT) wgmma_fence();
 #pragma unroll
@@ -522,7 +571,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
       uint32_t b_res = b_lo_base;
       for (int tap = 0; tap < taps; ++tap) {
         for (int cc = 0; cc < cchunks; ++cc) {
-          mbar_wait_parity(fullA(sa), pha);
+          mbar_wait_parity(stageA(sa), pha);
           uint32_t b_lo;
           if (RESIDENT) { b_lo = b_res; b_res += b_block16; }
           else { mbar_wait_parity(fullB(sb), phb); b_lo = b_lo_base + (uint32_t)sb * b_block16; }
@@ -586,9 +635,15 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             if (P.pow11_ch0 && n_off + c == 0) f0 = powf(1.1f, f0);   // cam scale channel (acr/model.py:95-96)
             if (resp) {
               float x0, x1;
-              unpack2<T>(*reinterpret_cast<const uint32_t*>(resp + c), x0, x1);
+              if constexpr (IsF32<T>::value) {
+                const float2 r = *reinterpret_cast<const float2*>(resp + c);
+                x0 = r.x; x1 = r.y;
+              } else {
+                unpack2<T>(*reinterpret_cast<const uint32_t*>(resp + c), x0, x1);
+              }
               f0 += x0; f1 += x1;
             }
+            if constexpr (!IsF32<T>::value)   // (extra terms: 16-bit plans only)
             for (int e = 0; e < P.n_ext; ++e) {   // folded fuse sum: the other terms, nearest-upsampled (warp-uniform loop)
               const T* xp = reinterpret_cast<const T*>(P.ext[e]) +
                             (((size_t)n * P.ext_H[e] + (oy >> P.ext_shift[e])) * P.ext_W[e] + (ox >> P.ext_shift[e])) * P.ext_stride[e] + n_off + c;
@@ -598,7 +653,9 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
             }
             if (P.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
           }
-          if (tma_out) {   // 16-byte chunk jj of the 128-byte row lives at chunk jj ^ (row & 7) (row & 7 = lane / 4)
+          if constexpr (IsF32<T>::value) {
+            *reinterpret_cast<float2*>(reinterpret_cast<float*>(P.out) + pix * P.out_stride + n_off + c) = make_float2(f0, f1);
+          } else if (tma_out) {   // 16-byte chunk jj of the 128-byte row lives at chunk jj ^ (row & 7) (row & 7 = lane / 4)
             sts32(srow + (((uint32_t)jj ^ (uint32_t)(lane >> 2)) << 4) + (uint32_t)cq * 2u, pack2<T>(f0, f1));
           } else if (P.out_f32) {
             *reinterpret_cast<float2*>(reinterpret_cast<float*>(P.out) + pix * P.out_stride + n_off + c) = make_float2(f0, f1);
@@ -656,7 +713,13 @@ static int launch_inst(const ConvTcPlan* pl, cudaStream_t st) {
 template <int CK, typename T>
 static int launch_mode(const ConvTcPlan* pl, cudaStream_t st) {
   const int mode = (pl->p.patch_mode ? MODE_PATCH : 0) | (pl->p.b_resident ? MODE_RESIDENT : 0);
-  if constexpr (CK == 64) {
+  if constexpr (IsF32<T>::value) {   // tf32: the single-box form and the four generic modes
+    if (pl->p.deconv || pl->p.s2x || pl->p.xpair) { set_error("conv_tc: no tf32 form of the transposed or x-paired convs"); return ACR_B200_EINVAL; }
+    if constexpr (CK == 64)
+      if (pl->p.patch1)
+        return pl->p.b_resident ? launch_inst<64, T, MODE_PATCH | MODE_RESIDENT | MODE_P1>(pl, st)
+                                : launch_inst<64, T, MODE_PATCH | MODE_P1>(pl, st);
+  } else if constexpr (CK == 64) {
     if (pl->p.deconv) return launch_inst<64, T, MODE_DECONV>(pl, st);
     if (pl->p.s2x)
       return pl->p.b_resident ? launch_inst<64, T, MODE_RESIDENT | MODE_S2X>(pl, st) : launch_inst<64, T, MODE_S2X>(pl, st);
@@ -681,5 +744,6 @@ int conv_tc_launch_64_bf16(const ConvTcPlan* pl, cudaStream_t st);
 int conv_tc_launch_64_f16(const ConvTcPlan* pl, cudaStream_t st);
 int conv_tc_launch_32(const ConvTcPlan* pl, cudaStream_t st);
 int conv_tc_launch_16(const ConvTcPlan* pl, cudaStream_t st);
+int conv_tc_launch_tf32(const ConvTcPlan* pl, cudaStream_t st);   // T = float, CK = 64 and 32
 
 }  // namespace acr

@@ -12,7 +12,7 @@ struct TensorRef {         // resolved acr_b200_tensor: absolute base pointer, p
 
 struct ConvArgs {
   TensorRef in, out, res;
-  const void* w;           // [cout_pad][k*k][cin_pad] 16-bit
+  const void* w;           // [cout_pad][k*k][cin_pad] 16-bit (fp32 in the TF32 plan)
   const float* bias;       // [cout_pad] (or [B][cout_pad] when bias_per_image)
   int k, stride, relu, has_res, cin_pad, cout_pad, bias_per_image, pow11_ch0, batch;
   int xpair;               // weights are the x-paired expansion of a 32->32 conv (ACR_CONV_XPAIR): side taps are 32x32 corners

@@ -4,6 +4,7 @@
 // schedule: tensor maps built once, branch-level concurrency on plan-internal streams, no Python
 // in the loop.  Also hosts the BN-folding weight packer.
 #include <stdlib.h>
+#include <string.h>
 #include <new>
 #include <vector>
 
@@ -111,9 +112,20 @@ static int run_one_f32(const acr_b200_op& op, int batch, char* arena, const char
   }
 }
 
+// a tensor record never says ACR_DT_TF32: the TF32 plan stores fp32 (ACR_DT_F32)
+static int check_tensor_dtypes(const acr_b200_op& op) {
+  bool ok = op.out.dtype != ACR_DT_TF32;
+  for (int i = 0; i < 4; ++i) ok = ok && op.aux[i].dtype != ACR_DT_TF32 && (i >= op.n_in || op.in[i].dtype != ACR_DT_TF32);
+  ACR_CHECK_ARG(ok, "op kind %d: ACR_DT_TF32 is an act_dtype, not a tensor dtype (the TF32 plan stores fp32)", op.kind);
+  return ACR_B200_OK;
+}
+
+// the plan of each act_dtype: the validation plan runs everything on validate_f32.cu; the TF32 plan only its convs on
+// the tensor cores (tf32 conv_tc instances); the part head is the same kernel in every plan
 static int run_one(const acr_b200_op& op, int batch, char* arena, const char* weights, const char* external,
                    int act_dtype, const ConvTcPlan* tc, cudaStream_t st) {
-  if (act_dtype == ACR_DT_F32 && op.kind != ACR_OP_PARTHEAD) return run_one_f32(op, batch, arena, weights, external, st);
+  const bool f32_kernels = act_dtype == ACR_DT_F32 || (act_dtype == ACR_DT_TF32 && op.kind != ACR_OP_CONV);
+  if (f32_kernels && op.kind != ACR_OP_PARTHEAD) return run_one_f32(op, batch, arena, weights, external, st);
   switch (op.kind) {
     case ACR_OP_STEM: {
       ACR_CHECK_ARG(external != nullptr, "stem: external image pointer is null");
@@ -227,8 +239,8 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
                                     size_t arena_bytes, const void* weights, size_t weight_bytes,
                                     int act_dtype, acr_b200_plan** plan_out) {
   ACR_CHECK_ARG(ops && n_ops > 0 && batch > 0 && arena && weights && plan_out, "plan_create: bad arguments");
-  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16 || act_dtype == ACR_DT_F32,
-                "plan_create: act_dtype must be bf16/f16 (product) or f32 (validation plan)");
+  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16 || act_dtype == ACR_DT_F32 || act_dtype == ACR_DT_TF32,
+                "plan_create: act_dtype must be bf16/f16 (product), f32 (validation plan) or tf32 (TF32 plan)");
   acr_b200_plan* p = new (std::nothrow) acr_b200_plan();
   ACR_CHECK_ARG(p != nullptr, "plan_create: out of host memory");
   p->ops.assign(ops, ops + n_ops);
@@ -244,13 +256,15 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
     const acr_b200_op& op = p->ops[i];
     if (op.stream_id < 0 || op.stream_id >= MAX_STREAMS) { set_error("op %d: stream_id out of range", i); rc = ACR_B200_EINVAL; break; }
     if (op.stream_id + 1 > p->n_streams) p->n_streams = op.stream_id + 1;
+    if ((rc = check_tensor_dtypes(op)) != ACR_B200_OK) break;
     if (!op.out.external && op.kind != ACR_OP_COORD) {
       const size_t esz = op.out.dtype == ACR_DT_F32 ? 4 : (op.out.dtype == ACR_DT_U8 ? 1 : 2);
       const size_t need = op.out.offset + (size_t)batch * op.out.H * op.out.W * op.out.pix_stride * esz;
       if (need > arena_bytes) { set_error("op %d: output exceeds the arena (%zu > %zu)", i, need, arena_bytes); rc = ACR_B200_EINVAL; break; }
     }
     if (p->fused[i]) continue;
-    if (op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32 && (op.shift[0] & ACR_CONV_BLOCK) && fuse_blocks_enabled()) {
+    const bool tc_conv = op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32;   // (the TF32 plan ignores ACR_CONV_BLOCK)
+    if (tc_conv && act_dtype != ACR_DT_TF32 && (op.shift[0] & ACR_CONV_BLOCK) && fuse_blocks_enabled()) {
       // one launch for the BasicBlock of ops i and i + 1 (the engine marks only such pairs); op i + 1's waits must be
       // ones op i already has, so nothing that op i + 1 waited for can be missed
       if (!(i + 1 < n_ops && p->ops[i + 1].kind == ACR_OP_CONV && p->ops[i + 1].stream_id == op.stream_id &&
@@ -266,7 +280,7 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
       p->fused[i + 1] = 1;
       continue;
     }
-    if (op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32) {
+    if (tc_conv) {
       ConvArgs a;
       rc = make_conv_args(op, batch, p->arena, p->weights, nullptr, &a);
       if (rc == ACR_B200_OK) rc = conv_tc_prepare(a, act_dtype, &p->tc[i]);
@@ -406,8 +420,21 @@ extern "C" void acr_b200_plan_destroy(acr_b200_plan* p) {
 extern "C" int acr_b200_run_op(const acr_b200_op* op, int batch, void* arena, const void* weights,
                                const void* external, int act_dtype, void* stream) {
   ACR_CHECK_ARG(op && batch > 0 && arena, "run_op: bad arguments");
+  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16 || act_dtype == ACR_DT_F32 || act_dtype == ACR_DT_TF32,
+                "run_op: act_dtype");
+  const int rc = check_tensor_dtypes(*op);
+  if (rc) return rc;
   return run_one(*op, batch, static_cast<char*>(arena), static_cast<const char*>(weights),
                  static_cast<const char*>(external), act_dtype, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+// nearest tf32 value of v, ties away from zero (cvt.rna.tf32.f32): low 13 mantissa bits cleared.  Inf / NaN pass through.
+static float round_tf32(float v) {
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  if ((u & 0x7f800000u) != 0x7f800000u) u = (u + 0x1000u) & ~0x1fffu;
+  memcpy(&v, &u, 4);
+  return v;
 }
 
 // BN folding + repack, host side.  y = gamma*(conv(x)+cb-mean)/sqrt(var+eps)+beta = conv'(x) + b'
@@ -416,7 +443,8 @@ extern "C" int acr_b200_pack_conv(const float* w, const float* conv_bias, const 
                                   int cout_pad, int cin_pad, int act_dtype, void* w_packed, float* bias_out) {
   ACR_CHECK_ARG(w && w_packed && bias_out && cout > 0 && cin > 0 && cout_pad >= cout && cin_pad >= cin,
                 "pack_conv: bad arguments");
-  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16 || act_dtype == ACR_DT_F32, "pack_conv: dtype");
+  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16 || act_dtype == ACR_DT_F32 || act_dtype == ACR_DT_TF32,
+                "pack_conv: dtype");
   const int taps = k * k;
   for (int co = 0; co < cout_pad; ++co) {
     float scale = 1.f, shift = 0.f;
@@ -432,6 +460,7 @@ extern "C" int acr_b200_pack_conv(const float* w, const float* conv_bias, const 
         const size_t idx = ((size_t)co * taps + t) * cin_pad + ci;
         if (act_dtype == ACR_DT_BF16) static_cast<__nv_bfloat16*>(w_packed)[idx] = __float2bfloat16_rn(v);
         else if (act_dtype == ACR_DT_F16) static_cast<__half*>(w_packed)[idx] = __float2half_rn(v);
+        else if (act_dtype == ACR_DT_TF32) static_cast<float*>(w_packed)[idx] = round_tf32(v);
         else static_cast<float*>(w_packed)[idx] = v;
       }
   }

@@ -278,7 +278,8 @@ enum {
 };  /* kinds stay below 16: acr_b200_plan_profile indexes ms_by_kind[16] */
 enum { ACR_CONV_BIAS_PER_IMAGE = 1, ACR_CONV_POW11_CH0 = 2, ACR_CONV_XPAIR = 4, ACR_CONV_S2X = 8, ACR_CONV_EXTRA = 16,
        ACR_CONV_DECONV = 32, ACR_CONV_BLOCK = 64, ACR_CONV_BLOCK_MID = 128 };
-enum { ACR_DT_BF16 = 0, ACR_DT_F16 = 1, ACR_DT_F32 = 2, ACR_DT_U8 = 3 };
+enum { ACR_DT_BF16 = 0, ACR_DT_F16 = 1, ACR_DT_F32 = 2, ACR_DT_U8 = 3,
+       ACR_DT_TF32 = 4 /* an act_dtype only (plan_create, run_op, pack_conv): fp32 storage, tf32 tensor-core convs */ };
 
 typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image extents)  */
   uint64_t offset;                /* byte offset of element (0,0,0,0) from the arena base   */
@@ -360,7 +361,20 @@ typedef struct acr_b200_plan acr_b200_plan;
 /* Build a launch plan for `batch` images.  `arena` (device, `arena_bytes`) holds every
  * activation; `weights` (device) the packed weight blob; ops are copied.  Creates the TMA
  * tensor maps and internal streams/events.  Replaces the module tree construction +
- * forward dispatch of acr/model.py:23-65 (ACR), :691-865 (HigherResolutionNet).           */
+ * forward dispatch of acr/model.py:23-65 (ACR), :691-865 (HigherResolutionNet).
+ * act_dtype:
+ *   ACR_DT_BF16 / ACR_DT_F16  the product plans: 16-bit activations and weights, fp32 accumulation on the tensor cores.
+ *   ACR_DT_F32                the validation plan: fp32 storage, fp64 accumulation on the CUDA cores (every op).
+ *   ACR_DT_TF32               the TF32 plan -- what an fp32 PyTorch model runs on Ampere / Hopper with cuDNN's default
+ *                             allow_tf32: fp32 storage (tensor records still say ACR_DT_F32) and fp32 outputs, every
+ *                             ACR_OP_CONV on the wgmma tensor cores with tf32 operands and fp32 accumulation.  Weights
+ *                             come from acr_b200_pack_conv(..., ACR_DT_TF32); the kernel rounds activations to the nearest
+ *                             tf32 in shared memory (storage stays fp32).  Every other
+ *                             op (stem, fuse, bilinear, coord, pooling, CONV_REF) runs on the validation plan's kernels,
+ *                             the part head as in every plan.  ACR_CONV_BLOCK marks are ignored (two resident fp32 weight
+ *                             sets do not fit the fused BasicBlock's shared memory), and the x-paired, stride-2 x-paired
+ *                             and transposed conv forms are ACR_B200_EINVAL.
+ * A tensor record whose dtype is ACR_DT_TF32 is ACR_B200_EINVAL (here and in acr_b200_run_op).                           */
 int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch, void* arena,
                          size_t arena_bytes, const void* weights, size_t weight_bytes,
                          int act_dtype, acr_b200_plan** plan_out);
@@ -383,13 +397,16 @@ int acr_b200_plan_num_launches(const acr_b200_plan* plan);
 int acr_b200_plan_op_launch(const acr_b200_plan* plan, int32_t* launch_of_op);
 void acr_b200_plan_destroy(acr_b200_plan* plan);
 
-/* Single-op entry used by the parity tests (same code path as inside a plan).             */
+/* Single-op entry used by the parity tests (same code path as inside a plan, any act_dtype of plan_create).      */
 int acr_b200_run_op(const acr_b200_op* op, int batch, void* arena, const void* weights,
                     const void* external, int act_dtype, void* stream);
 
 /* Host-side weight folding/packing for one conv (acr_b200_weights_pack of SURVEY.md 8b):
  * folds eval-mode BatchNorm (acr/model.py BN after every conv) into w/b and repacks
- * OIHW fp32 -> [cout_pad][kh][kw][cin_pad] 16-bit (K-major rows for the wgmma B operand).
+ * OIHW fp32 -> [cout_pad][kh][kw][cin_pad] 16-bit (K-major rows for the wgmma B operand),
+ * or fp32 for ACR_DT_F32 and ACR_DT_TF32.  ACR_DT_TF32 packs exactly like ACR_DT_F32, then
+ * rounds every weight to the nearest tf32 value (ties away from zero, as cvt.rna.tf32.f32):
+ * its low 13 mantissa bits are zero.  The bias is fp32 in every mode.
  * bn_* may be NULL (no BN); conv_bias may be NULL.  All pointers are HOST pointers.       */
 int acr_b200_pack_conv(const float* w_oihw, const float* conv_bias, const float* bn_gamma,
                        const float* bn_beta, const float* bn_mean, const float* bn_var, float bn_eps,
