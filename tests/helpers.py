@@ -54,9 +54,16 @@ def u16_to_float(a: np.ndarray, dt) -> torch.Tensor:
     return t.view(torch.bfloat16 if dt == L.DT_BF16 else torch.float16).float()
 
 
+CONV_BIAS_PER_IMAGE, CONV_POW11_CH0 = 1, 2     # ACR_CONV_* flag bits (shift[0]) of a CONV op
+
+
 def run_conv_case(kind, B, H, W, cin, cout, k, s, relu, residual, bias, bn, out_f32, dt=L.DT_BF16, seed=0,
-                  in_stride=None, cin_pad=None):
-    """Runs one conv through acr_b200_run_op on the GPU and returns (got, expected) fp32 NCHW."""
+                  in_stride=None, cin_pad=None, flags=0, bias_img=None):
+    """Runs one conv through acr_b200_run_op on the GPU and returns (got, expected) fp32 NCHW.
+
+    flags: ACR_CONV_* bits of the op.  With CONV_BIAS_PER_IMAGE the bias is ``bias_img``, an fp32 (B, cout_pad) tensor
+    placed in the arena as aux[0] (the folded part-head conv).  With any flag the expected output is computed in fp64 on
+    the same rounded operands, in the kernel's epilogue order: + bias, 1.1 ** channel 0, + residual, ReLU."""
     import torch.nn.functional as Fn
     g = torch.Generator().manual_seed(seed)
     tdt = torch.bfloat16 if dt == L.DT_BF16 else torch.float16
@@ -83,7 +90,13 @@ def run_conv_case(kind, B, H, W, cin, cout, k, s, relu, residual, bias, bn, out_
     off_o = rup(off_r + rbytes, 1024)
     oesz = 4 if out_f32 else 2
     obytes = B * Ho * Wo * cout_pad * oesz
-    arena = torch.zeros(off_o + obytes + 1024, dtype=torch.uint8)
+    per_image = bool(flags & CONV_BIAS_PER_IMAGE)
+    if per_image:
+        assert bias_img is not None and tuple(bias_img.shape) == (B, cout_pad) and bias_img.dtype == torch.float32
+    off_b = rup(off_o + obytes, 1024)
+    arena = torch.zeros(off_b + (B * cout_pad * 4 if per_image else 0) + 1024, dtype=torch.uint8)
+    if per_image:
+        arena[off_b: off_b + B * cout_pad * 4] = bias_img.contiguous().view(torch.uint8).flatten()
     arena[off_x: off_x + xin.numel() * esz] = xin.view(torch.uint8).flatten()
     if residual:
         rin = to_nhwc_padded(res, res_stride, tdt)
@@ -98,9 +111,12 @@ def run_conv_case(kind, B, H, W, cin, cout, k, s, relu, residual, bias, bn, out_
     if residual:
         op.in_[1] = ctensor(off_r, cout, Ho, Wo, res_stride, dt)
     op.out = ctensor(off_o, cout, Ho, Wo, cout_pad, L.DT_F32 if out_f32 else dt)
+    if per_image:
+        op.aux[0] = ctensor(off_b, cout_pad, 1, 1, cout_pad, L.DT_F32)
     op.w_offset[0], op.w_offset[1] = w_off, b_off
     op.k, op.stride, op.relu, op.has_residual = k, s, int(relu), int(residual)
     op.cin_pad, op.cout_pad = cin_pad, cout_pad
+    op.shift[0] = flags
     d_arena = arena.cuda()
     d_blob = torch.from_numpy(blob).cuda()
     lib = L.load()
@@ -111,10 +127,16 @@ def run_conv_case(kind, B, H, W, cin, cout, k, s, relu, residual, bias, bn, out_
     got = raw.view(torch.float32 if out_f32 else tdt).view(B, Ho, Wo, cout_pad).float()
     pad_ok = bool((got[..., cout:] == 0).all())
     got = got[..., :cout].permute(0, 3, 1, 2).contiguous()
-    # expected: same rounded operands, fp32 math on the CPU
+    # expected: same rounded operands, fp32 math on the CPU (fp64 with flags)
     wf = u16_to_float(wp, dt).view(cout_pad, k, k, cin_pad)[:cout, :, :, :cin].permute(0, 3, 1, 2).contiguous()
     xf = xin[..., :cin].float().permute(0, 3, 1, 2).contiguous()
-    exp = Fn.conv2d(xf, wf, torch.from_numpy(bvec[:cout].copy()), s, k // 2)
+    if flags:
+        exp = Fn.conv2d(xf.double(), wf.double(), None, s, k // 2)
+        exp = exp + (bias_img[:, :cout, None, None] if per_image else torch.from_numpy(bvec[:cout].copy()).view(1, -1, 1, 1)).double()
+        if flags & CONV_POW11_CH0:
+            exp = torch.cat([torch.pow(1.1, exp[:, :1]), exp[:, 1:]], 1)
+    else:
+        exp = Fn.conv2d(xf, wf, torch.from_numpy(bvec[:cout].copy()), s, k // 2)
     if residual:
         exp = exp + rin[..., :cout].float().permute(0, 3, 1, 2)
     if relu:

@@ -315,7 +315,11 @@ def test_full_batch_256_is_batch_invariant(sd, image):
     """BASELINE configs[2] size (256 frames per GPU) through a size-independent property: every kernel of the plan
     works per image (conv super-tiles, pooling chunks, part head), so a frame's maps must not depend on the
     batch it travels in -- the 256-frame plan run on the two test frames repeated 128 times reproduces the
-    2-frame plan (itself pinned against the oracle above) bit for bit, at every position of the batch."""
+    2-frame plan (itself pinned against the oracle above) bit for bit, at every position of the batch.
+    What this does NOT cover: a kernel that takes image b's per-image data (bias, pooling partials, part-head offsets,
+    batch coordinate) from another image is wrong in the same way in both plans, and the 2-frame plan is pinned against
+    the oracle only at TOL_NET.  Distinct frames, batch-1 parity of every plan and every launch, and a permuted
+    256-frame batch are in tests/test_gpu_batch.py."""
     from acr_b200.engine import Engine
     B = 256
     names = ["segms", "l_center_map", "r_center_map", "l_params_maps", "r_params_maps", "l_prior_maps", "r_prior_maps"]

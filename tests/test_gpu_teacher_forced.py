@@ -25,8 +25,9 @@ def sd():
 
 @pytest.fixture(scope="module")
 def image():
-    # one frame: the sweep re-computes every op on the CPU, and every kernel works per image (the batch dimension is
-    # covered by tests/test_gpu_network.py::test_full_batch_256_is_batch_invariant)
+    # one frame: the sweep re-computes every op on the CPU.  At batch 1 a kernel that reads another image's data reads its
+    # own; the batch dimension is covered by tests/test_gpu_batch.py (every op teacher forced on three distinct frames,
+    # every launch per image against batch 1)
     gi = torch.Generator().manual_seed(123)
     return torch.randint(0, 256, (2, 512, 512, 3), generator=gi, dtype=torch.uint8)[1:]
 
