@@ -107,6 +107,38 @@ class ACR(nn.Module):
         return replay
 
     @torch.no_grad()
+    def capture_frames_graph(self, batch: int, max_frame_bytes: int, device=None):
+        """``capture_graph`` from raw frames: one CUDA graph of the ragged pre-processing (cubic tables, BGR->RGB,
+        white pad, bicubic resize, offsets; acr_b200.preprocess.RaggedFrames) followed by ``fused_forward``.  Returns
+        ``replay(frames) -> (bufs, mano)`` for a list of exactly ``batch`` BGR frames (numpy arrays, CPU or CUDA
+        tensors) of any sizes, each replay its own, whose packed H*W*3 bytes sum to at most ``max_frame_bytes``.  Host
+        frames travel in one H2D copy; a list that does not fit raises before anything is enqueued."""
+        from acr_b200.preprocess import RaggedFrames
+        import numpy as np
+        dev = torch.device(device) if device is not None else next(self.model.parameters()).device
+        rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
+            rf.load([np.full((1, 1, 3), 255, np.uint8)] * batch)
+            for _ in range(2):
+                self.fused_forward(*rf.launch())
+        cur.wait_stream(side)
+        torch.cuda.synchronize(dev)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            bufs, mano = self.fused_forward(*rf.launch())
+
+        def replay(frames):
+            rf.load(frames)
+            graph.replay()
+            return bufs, mano
+
+        replay.graph, replay.frames = graph, rf
+        return replay
+
+    @torch.no_grad()
     def single_image_forward(self, image_rgb_u8_512, path=None):
         meta = {'image': image_rgb_u8_512[None] if image_rgb_u8_512.dim() == 3 else image_rgb_u8_512,
                 'offsets': torch.tensor([[512., 512, 0, 0, 0, 0, 0, 0, 0, 0]]), 'batch_ids': torch.arange(1)}

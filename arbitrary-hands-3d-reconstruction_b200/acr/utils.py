@@ -118,9 +118,22 @@ def save_results(image_folder, output_dir, results_dict):
 def img_preprocess(image, imgpath=None, input_size=512, single_img_input=False, bbox=None):
     """Drop-in for acr/utils.py:1315-1337 on the device: ``image`` is a BGR frame (numpy HxWx3 uint8, or a CUDA
     uint8 tensor HxWx3 / NxHxWx3); returns the reference's dict with ``image`` (uint8 RGB, white-padded to a
-    square and bicubic-resized to input_size) as a CUDA tensor and the 10-element ``offsets``."""
+    square and bicubic-resized to input_size) as a CUDA tensor and the 10-element ``offsets``.
+
+    ``image`` may also be a list of BGR frames of any sizes (numpy arrays, CPU or CUDA tensors): they are resized in
+    one launch, ``image`` is then (n, S, S, 3) and ``offsets`` (n, 10), each row in its own frame's pixels, and a list
+    ``imgpath`` gives lists ``imgpath`` and ``name``."""
     from acr_b200.preprocess import preprocess_frames
     import numpy as np
+    if isinstance(image, (list, tuple)):
+        paths = None if imgpath is None else [imgpath] if isinstance(imgpath, str) else list(imgpath)
+        if paths is not None and len(paths) != len(image):
+            raise ValueError(f"{len(image)} frames but {len(paths)} image paths")
+        out, offsets = preprocess_frames(list(image), input_size)
+        input_data = {'image': out, 'offsets': offsets, 'data_set': 'internet'}
+        if paths is not None:
+            input_data.update({'imgpath': paths, 'name': [os.path.basename(p) for p in paths]})
+        return input_data
     t = torch.from_numpy(np.ascontiguousarray(image)) if isinstance(image, np.ndarray) else image
     t = t.cuda(non_blocking=True)
     batched = t.dim() == 4

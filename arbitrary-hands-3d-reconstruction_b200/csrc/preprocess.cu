@@ -58,6 +58,101 @@ __global__ void __launch_bounds__(256) preprocess_kernel(PreArgs a) {
   for (int c = 0; c < 3; ++c) o[c] = (uint8_t)min(max((acc[c] + (1 << 21)) >> 22, 0), 255);
 }
 
+// ---- ragged batches: per-frame geometry and tables are device data ------------------------------------------------
+// acr_b200/preprocess.py::cubic_tables, one thread per (frame, d).  Every operation is the numpy one, rounded to
+// nearest on its own: fx in double, then the A = -0.75 polynomials in float32 left to right (numpy's order), so
+// nothing may be contracted into an FMA.  5A, 8A, 4A, A+2 and A+3 are exact in float32.
+__global__ void __launch_bounds__(256) cubic_tables_kernel(const int32_t* n_src, int n, int S, int16_t* coef,
+                                                           int32_t* ofs) {
+  const long long gid = (long long)blockIdx.x * 256 + threadIdx.x;
+  if (gid >= (long long)n * S) return;
+  const int src = n_src[gid / S], d = (int)(gid % S);
+  int16_t* c_out = coef + gid * 4;
+  if (src < 1) {
+    c_out[0] = c_out[1] = c_out[2] = c_out[3] = 0;
+    ofs[gid] = 0;
+    return;
+  }
+  const double scale = __ddiv_rn((double)src, (double)S);
+  const float fx = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
+  const float s = floorf(fx);
+  const float x = __fsub_rn(fx, s);
+  const float x1 = __fadd_rn(x, 1.f), u = __fsub_rn(1.f, x);
+  float c[4];
+  c[0] = __fsub_rn(__fmul_rn(__fadd_rn(__fmul_rn(__fsub_rn(__fmul_rn(-0.75f, x1), -3.75f), x1), -6.f), x1), -3.f);
+  c[1] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(1.25f, x), 2.25f), x), x), 1.f);
+  c[2] = __fadd_rn(__fmul_rn(__fmul_rn(__fsub_rn(__fmul_rn(1.25f, u), 2.25f), u), u), 1.f);
+  c[3] = __fsub_rn(__fsub_rn(__fsub_rn(1.f, c[0]), c[1]), c[2]);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) c_out[k] = (int16_t)rintf(__fmul_rn(c[k], 2048.f));
+  ofs[gid] = (int32_t)s;
+}
+
+struct RaggedArgs {
+  const uint8_t* src;               // packed BGR frames, src_bytes bytes
+  long long src_bytes;
+  const acr_b200_frame* frames;     // (n)
+  const int16_t* coef;              // (n,S,4), both axes of a frame
+  const int32_t* ofs;               // (n,S)
+  uint8_t* dst;                     // (n,S,S,3) RGB
+  float* offsets;                   // (n,10) or null
+  int S;
+};
+
+// side - H and side - W are >= 0 once side == max(H, W), so no sum below can overflow
+__device__ __forceinline__ bool frame_ok(const acr_b200_frame& f, long long src_bytes) {
+  return f.H >= 1 && f.W >= 1 && f.side == max(f.H, f.W) && f.pad_t >= 0 && f.pad_l >= 0 &&
+         f.pad_t <= f.side - f.H && f.pad_l <= f.side - f.W && f.offset >= 0 && f.offset <= src_bytes &&
+         (long long)f.H * f.W <= (src_bytes - f.offset) / 3;
+}
+
+// grid (pixel blocks, n): blockIdx.y is the frame.  Per pixel the arithmetic of preprocess_kernel.
+__global__ void __launch_bounds__(256) preprocess_ragged_kernel(RaggedArgs a) {
+  const int img = blockIdx.y, S = a.S;
+  const acr_b200_frame f = a.frames[img];
+  const bool ok = frame_ok(f, a.src_bytes);
+  if (a.offsets && blockIdx.x == 0 && threadIdx.x < 10) {
+    const int i = threadIdx.x;
+    const int v = !ok ? 0 : i < 2 ? f.side : i == 6 ? f.pad_t : i == 7 ? f.side - f.W - f.pad_l
+                : i == 8 ? f.side - f.H - f.pad_t : i == 9 ? f.pad_l : 0;
+    a.offsets[img * 10 + i] = (float)v;
+  }
+  const int pix = blockIdx.x * 256 + threadIdx.x;
+  if (pix >= S * S) return;
+  uint8_t* o = a.dst + ((size_t)img * S * S + pix) * 3;
+  if (!ok) {
+    o[0] = o[1] = o[2] = 0;
+    return;
+  }
+  const int dx = pix % S, dy = pix / S;
+  const int16_t* cf = a.coef + (size_t)img * S * 4;
+  const int32_t* of = a.ofs + (size_t)img * S;
+  const uint8_t* src = a.src + f.offset;
+  int acc[3] = {0, 0, 0};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const int py = min(max(of[dy] + j - 1, 0), f.side - 1);   // replicate border of the padded square
+    const int sy = py - f.pad_t;
+    int hor[3] = {0, 0, 0};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int px = min(max(of[dx] + k - 1, 0), f.side - 1);
+      const int sx = px - f.pad_l;
+      const int w = cf[dx * 4 + k];
+      if (sy >= 0 && sy < f.H && sx >= 0 && sx < f.W) {
+        const uint8_t* p = src + ((size_t)sy * f.W + sx) * 3;
+        hor[0] += w * p[2]; hor[1] += w * p[1]; hor[2] += w * p[0];   // BGR -> RGB
+      } else {
+        hor[0] += w * 255; hor[1] += w * 255; hor[2] += w * 255;      // white padding
+      }
+    }
+    const int wy = cf[dy * 4 + j];
+    acc[0] += wy * hor[0]; acc[1] += wy * hor[1]; acc[2] += wy * hor[2];
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c] = (uint8_t)min(max((acc[c] + (1 << 21)) >> 22, 0), 255);
+}
+
 }  // namespace acr
 
 using namespace acr;
@@ -71,6 +166,31 @@ extern "C" int acr_b200_preprocess(const uint8_t* frames_bgr, int n, int H, int 
   PreArgs a{frames_bgr, out_rgb, coef_x, ofs_x, coef_y, ofs_y, n, H, W, out_size, side, pad_t, pad_l};
   const long long total = (long long)n * out_size * out_size;
   preprocess_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}
+
+extern "C" int acr_b200_cubic_tables(const int32_t* n_src, int n, int out_size, int16_t* coef, int32_t* ofs,
+                                     void* stream) {
+  ACR_CHECK_ARG(n_src && coef && ofs, "cubic_tables: null argument");
+  const long long total = (long long)n * out_size;
+  ACR_CHECK_ARG(n > 0 && out_size > 0 && (total + 255) / 256 <= 0x7fffffff, "cubic_tables: bad n=%d / out_size=%d",
+                n, out_size);
+  cubic_tables_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(n_src, n, out_size, coef, ofs);
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}
+
+extern "C" int acr_b200_preprocess_ragged(const uint8_t* frames_bgr, int64_t src_bytes, const acr_b200_frame* frames,
+                                          int n, const int16_t* coef, const int32_t* ofs, int out_size,
+                                          uint8_t* out_rgb, float* offsets, void* stream) {
+  ACR_CHECK_ARG(frames_bgr && frames && coef && ofs && out_rgb, "preprocess_ragged: null argument");
+  // grid.y carries the frame; S * S must fit the int pixel index
+  ACR_CHECK_ARG(n > 0 && n <= 65535 && out_size > 0 && out_size <= 16384 && src_bytes >= 0,
+                "preprocess_ragged: bad n=%d / out_size=%d / src_bytes=%lld", n, out_size, (long long)src_bytes);
+  RaggedArgs a{frames_bgr, (long long)src_bytes, frames, coef, ofs, out_rgb, offsets, out_size};
+  const dim3 grid((unsigned)(((long long)out_size * out_size + 255) / 256), (unsigned)n);
+  preprocess_ragged_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a);
   ACR_CHECK_LAUNCH();
   return ACR_B200_OK;
 }

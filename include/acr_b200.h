@@ -199,6 +199,33 @@ int acr_b200_preprocess(const uint8_t* frames_bgr, int n, int H, int W, const in
                         const int32_t* ofs_x, const int16_t* coef_y, const int32_t* ofs_y, int side, int pad_t,
                         int pad_l, int out_size, uint8_t* out_rgb, void* stream);
 
+/* The cubic tables of acr_b200/preprocess.py::cubic_tables on the device, for n source squares at once: frame i
+ * (side n_src[i], device int32) gets coef[i] (out_size,4) int16 and ofs[i] (out_size) int32, bit for bit the host's
+ * float32 arithmetic (explicit round-to-nearest operations, no contraction).  One thread per (frame, d).  An
+ * n_src[i] < 1 gives zero tables.  Graph-capturable: a replay reads the sides it finds in n_src.            */
+int acr_b200_cubic_tables(const int32_t* n_src, int n, int out_size, int16_t* coef, int32_t* ofs, void* stream);
+
+/* One frame of a ragged batch: its BGR HWC bytes start `offset` bytes into the packed buffer; it is white-padded
+ * to a side x side square with pad_t rows above and pad_l columns to the left. 32 bytes. */
+typedef struct acr_b200_frame {
+  int64_t offset;
+  int32_t H, W, side, pad_t, pad_l;
+  int32_t reserved;  /* 0 */
+} acr_b200_frame;
+
+/* acr_b200_preprocess for n frames of any sizes in one launch (grid: pixel blocks x n).  `frames_bgr` holds
+ * src_bytes bytes: every frame back to back (HWC, contiguous), where frames[i] (device) says.  coef (n,out_size,4)
+ * and ofs (n,out_size) are frame i's tables for its side (acr_b200_cubic_tables), used on both axes.  Per-pixel
+ * arithmetic as acr_b200_preprocess.  Outputs out_rgb (n,out_size,out_size,3) and, when offsets is not NULL, the
+ * (n,10) fp32 offsets vectors [side, side, 0,0,0,0, pad_t, r, b, pad_l] of the descriptors.
+ * n < 1 or > 65535, out_size < 1, src_bytes < 0 or a NULL input is ACR_B200_EINVAL.  The descriptors are device
+ * data (a graph replay may change every frame's size), so they are checked on the device: a frame that breaks
+ * H, W >= 1, side = max(H, W), pad_t, pad_l >= 0, pad_t + H <= side, pad_l + W <= side, offset >= 0 or
+ * offset + H*W*3 <= src_bytes reads nothing and gets an all-zero image and offsets row.                  */
+int acr_b200_preprocess_ragged(const uint8_t* frames_bgr, int64_t src_bytes, const acr_b200_frame* frames, int n,
+                               const int16_t* coef, const int32_t* ofs, int out_size, uint8_t* out_rgb,
+                               float* offsets, void* stream);
+
 /* Temporal OneEuro smoothing of poses / betas between parse and MANO, in place, on the device
  * (SURVEY.md 8f-3).  Replaces OneEuroFilter / LowPassFilter (acr/utils.py:1485-1527), smooth_results
  * (:1478-1482), smooth_global_rot_matrix (:1466-1470) and the per-frame host loop of acr/main.py:69-83.
