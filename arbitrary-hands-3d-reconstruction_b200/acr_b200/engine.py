@@ -382,6 +382,41 @@ class Engine:
             recs[i]["block"] = True
             recs[i]["block_mid"] = not reuse_memory or recs[i]["out"].name in keep_roots
 
+        def bottleneck_triple(i) -> bool:
+            """recs i .. i + 2 are one Bottleneck that the fused kernel takes (csrc/conv_bottleneck.cuh): 1x1 C_in -> 64
+            (C_in 64 or 256), 3x3 64 -> 64, 1x1 64 -> 256 + residual, stride 1, ReLU on all three; the residual is the
+            block input or a downsample's output; and neither intermediate is observable (reuse_memory=False keeps
+            every tensor, keep_extra may name one): those triples stay three launches."""
+            if self.f32 or not reuse_memory or i + 2 >= len(recs):
+                return False
+            rs = recs[i: i + 3]
+            if any(r["kind"] != L.OP_CONV for r in rs):
+                return False
+            at = [r.get("attrs", {}) for r in rs]
+            special = ("extra", "merged", "fold_side", "stem", "deconv", "pow11")
+            if any(a.get(k) for a in at for k in special):
+                return False
+            if [(a.get("k"), a.get("s"), bool(a.get("relu")), bool(a.get("residual"))) for a in at] != \
+                    [(1, 1, True, False), (3, 1, True, False), (1, 1, True, True)]:
+                return False
+            x, y1, y2, out = rs[0]["ins"][0], rs[0]["out"], rs[1]["out"], rs[2]["out"]
+            if len(rs[1]["ins"]) != 1 or rs[1]["ins"][0] is not y1 or len(rs[2]["ins"]) != 2 or rs[2]["ins"][0] is not y2:
+                return False
+            res = rs[2]["ins"][1]
+            downsample = any(r["kind"] == L.OP_CONV and r["out"] is res and r["ins"][0] is x for r in recs[:i])
+            if res is not x and not downsample:
+                return False
+            ts = (x, y1, y2, out, res)
+            if not (x.C in (64, 256) and y1.C == y2.C == 64 and out.C == res.C == 256 and
+                    all(t.base is None and t.dtype == "act" for t in ts)):
+                return False
+            return all(y.name not in keep_roots and last_use[y.name] == j for y, j in ((y1, i + 1), (y2, i + 2)))
+
+        # Bottlenecks run as one launch each, kept apart from the BasicBlocks
+        self.bottleneck_starts = [i for i in range(len(recs)) if bottleneck_triple(i)]
+        for i in self.bottleneck_starts:
+            recs[i]["bottleneck"] = True
+
         if self.dry_run:
             return
 
@@ -487,6 +522,8 @@ class Engine:
                         o.shift[0] |= 2  # ACR_CONV_POW11_CH0
                 if r.get("block"):
                     o.shift[0] |= L.CONV_BLOCK | (L.CONV_BLOCK_MID if r["block_mid"] else 0)
+                if r.get("bottleneck"):
+                    o.shift[0] |= L.CONV_BOTTLENECK
             elif r["kind"] == L.OP_STEM_TC:
                 # weights (64,3,k,k) OIHW -> (64, K, 1, 1) with input channel (ky*k+kx)*3+ci, K = 32 (3x3) or 160 (7x7: k = 7
                 # in the op); BN folded by pack_conv
@@ -588,7 +625,8 @@ class Engine:
 
     def profile_ops(self, image: torch.Tensor) -> np.ndarray:
         """One serialised, event-bracketed pass: device ms of every record, in the order of ``recs``.  The two convs of a
-        fused BasicBlock are one launch: its time is on the first, the second reads 0 (``launch_of_rec``)."""
+        fused BasicBlock (or the three of a fused Bottleneck) are one launch: its time is on the first, the others read 0
+        (``launch_of_rec``)."""
         ms = np.zeros(self.n_ops, np.float32)
         with torch.cuda.device(self.device):
             L.check(self.lib.acr_b200_plan_profile_ops(self.plan, image.data_ptr(), self._stream(), ms.ctypes.data),
@@ -600,7 +638,7 @@ class Engine:
         return int(self.lib.acr_b200_plan_num_launches(self.plan))
 
     def launch_of_rec(self) -> np.ndarray:
-        """Index of the launch that computes each record (the two convs of a fused BasicBlock share one)."""
+        """Index of the launch that computes each record (the convs of a fused BasicBlock or Bottleneck share one)."""
         out = np.zeros(self.n_ops, np.int32)
         L.check(self.lib.acr_b200_plan_op_launch(self.plan, out.ctypes.data), "plan_op_launch")
         return out

@@ -19,6 +19,7 @@ OP_MAXPOOL = 12
 CONV_DECONV = 32      # ACR_CONV_DECONV flag bit (shift[0]) of a CONV op
 CONV_BLOCK = 64       # ACR_CONV_BLOCK: this conv and the next are one BasicBlock, run as one launch
 CONV_BLOCK_MID = 128  # ACR_CONV_BLOCK_MID: the fused launch also writes the block's intermediate
+CONV_BOTTLENECK = 256  # ACR_CONV_BOTTLENECK: this conv and the next two are one Bottleneck, run as one launch
 DT_BF16, DT_F16, DT_F32, DT_U8 = 0, 1, 2, 3
 DT_TF32 = 4           # act_dtype of the TF32 plan (plan_create / run_op / pack_conv only; its tensors are DT_F32)
 POSE_AXISANG, POSE_ROTMAT = 0, 1   # ACR_B200_POSE_*: pose input of acr_b200_mano_layer_forward / _backward / _jvp

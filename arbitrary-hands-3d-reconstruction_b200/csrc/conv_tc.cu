@@ -1,6 +1,7 @@
 // Host side of the implicit-GEMM conv (conv_tc.cuh): tensor maps, N split, shared-memory plan, launch dispatch; and of
-// the fused BasicBlock (conv_block.cuh).
+// the fused BasicBlock (conv_block.cuh) and Bottleneck (conv_bottleneck.cuh).
 #include "conv_block.cuh"
+#include "conv_bottleneck.cuh"
 
 namespace acr {
 
@@ -270,5 +271,60 @@ int conv_block_prepare(const ConvArgs& a1, const ConvArgs& a2, int act_dtype, in
 }
 
 void conv_block_free(ConvBlockPlan* p) { delete p; }
+
+int conv_bottleneck_prepare(const ConvArgs& a1, const ConvArgs& a2, const ConvArgs& a3, int act_dtype, ConvBottleneckPlan** out) {
+  auto plain = [&](const ConvArgs& a, int k, int cout_pad) {
+    return a.k == k && a.stride == 1 && a.cout_pad == cout_pad && a.relu && !a.bias_per_image && !a.pow11_ch0 && a.n_ext == 0 &&
+           !a.xpair && !a.s2x && !a.deconv && a.in.dtype == act_dtype && a.out.dtype == act_dtype;
+  };
+  ACR_CHECK_ARG(act_dtype == ACR_DT_BF16 || act_dtype == ACR_DT_F16, "conv_bottleneck: 16-bit activations only");
+  ACR_CHECK_ARG(plain(a1, 1, 64) && plain(a2, 3, 64) && plain(a3, 1, 256) && !a1.has_res && !a2.has_res && a3.has_res &&
+                    (a1.cin_pad == 64 || a1.cin_pad == 256) && a2.cin_pad == 64 && a3.cin_pad == 64 && a3.res.dtype == act_dtype,
+                "conv_bottleneck: 1x1 (64 or 256) -> 64, 3x3 64 -> 64, 1x1 64 -> 256 + residual, stride 1, ReLU on all three");
+  ACR_CHECK_ARG(a2.in.ptr == a1.out.ptr && a3.in.ptr == a2.out.ptr, "conv_bottleneck: each conv must read the previous one's output");
+  const int H = a1.in.H, W = a1.in.W;
+  ACR_CHECK_ARG(a1.out.H == H && a1.out.W == W && a2.out.H == H && a2.out.W == W && a3.out.H == H && a3.out.W == W &&
+                    H % TILE_Y == 0 && W % TILE_X == 0,
+                "conv_bottleneck: %dx%d is not a multiple of the 16x16 super-tile", H, W);
+  ACR_CHECK_ARG(a1.in.pix_stride % 8 == 0 && a1.in.pix_stride >= a1.cin_pad && a3.out.pix_stride % 2 == 0 && a3.out.pix_stride >= 256 &&
+                    a3.res.pix_stride % 2 == 0 && a3.res.pix_stride >= 256,
+                "conv_bottleneck: row alignment");
+  ConvBottleneckPlan* pl = new ConvBottleneckPlan();
+  ConvBottleneckParams& p = pl->p;
+  pl->act_dtype = act_dtype;
+  const cuuint64_t esz = 2;
+  int rc;
+  {
+    cuuint64_t dims[4] = {(cuuint64_t)a1.cin_pad, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)a1.batch};
+    cuuint64_t str[3] = {(cuuint64_t)a1.in.pix_stride * esz, (cuuint64_t)W * a1.in.pix_stride * esz,
+                         (cuuint64_t)H * W * a1.in.pix_stride * esz};
+    cuuint32_t box[4] = {64, BNK_PITCH, BNK_ROWS, 1};
+    rc = encode(&p.tmA, act_dtype, 4, a1.in.ptr, dims, str, box, 64);
+  }
+  // packed weights [cout_pad][taps * cin_pad]: conv1 [64][C_in], conv2 [64][9 * 64], conv3 [256][64] (one box)
+  const ConvArgs* as[3] = {&a1, &a2, &a3};
+  CUtensorMap* tms[3] = {&p.tmB1, &p.tmB2, &p.tmB3};
+  for (int c = 0; c < 3 && !rc; ++c) {
+    const ConvArgs& a = *as[c];
+    const cuuint64_t kk = (cuuint64_t)a.k * a.k * a.cin_pad;
+    cuuint64_t dims[2] = {kk, (cuuint64_t)a.cout_pad};
+    cuuint64_t str[1] = {kk * esz};
+    cuuint32_t box[2] = {64, (cuuint32_t)a.cout_pad};
+    rc = encode(tms[c], act_dtype, 2, a.w, dims, str, box, 64);
+  }
+  if (rc) { delete pl; return rc; }
+  p.bias1 = a1.bias; p.bias2 = a2.bias; p.bias3 = a3.bias;
+  p.res = a3.res.ptr; p.out = a3.out.ptr;
+  pl->cchunks = a1.cin_pad / 64;
+  p.res_stride = a3.res.pix_stride; p.out_stride = a3.out.pix_stride;
+  p.H = H; p.W = W;
+  p.tiles_x = W / TILE_X; p.tiles_per_img = p.tiles_x * (H / TILE_Y);
+  p.total_tiles = p.tiles_per_img * a1.batch;
+  pl->grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
+  *out = pl;
+  return ACR_B200_OK;
+}
+
+void conv_bottleneck_free(ConvBottleneckPlan* p) { delete p; }
 
 }  // namespace acr

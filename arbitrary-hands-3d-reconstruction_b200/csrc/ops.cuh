@@ -82,5 +82,10 @@ struct ConvBlockPlan;
 int conv_block_prepare(const ConvArgs& a1, const ConvArgs& a2, int act_dtype, int store_mid, ConvBlockPlan** out);
 int conv_block_launch(const ConvBlockPlan* p, cudaStream_t st);
 void conv_block_free(ConvBlockPlan* p);
+// one Bottleneck (1x1 C_in -> 64, 3x3 64 -> 64, 1x1 64 -> 256 + residual) as one launch (conv_bottleneck.cuh)
+struct ConvBottleneckPlan;
+int conv_bottleneck_prepare(const ConvArgs& a1, const ConvArgs& a2, const ConvArgs& a3, int act_dtype, ConvBottleneckPlan** out);
+int conv_bottleneck_launch(const ConvBottleneckPlan* p, cudaStream_t st);
+void conv_bottleneck_free(ConvBottleneckPlan* p);
 
 }  // namespace acr

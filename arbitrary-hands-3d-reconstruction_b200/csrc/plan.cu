@@ -210,7 +210,8 @@ struct acr_b200_plan {
   std::vector<acr_b200_op> ops;
   std::vector<ConvTcPlan*> tc;
   std::vector<ConvBlockPlan*> blk;     // op i (ACR_CONV_BLOCK) launches the fused BasicBlock of ops i and i + 1
-  std::vector<char> fused;             // op i is the second conv of a fused block: no launch of its own
+  std::vector<ConvBottleneckPlan*> bnk;   // op i (ACR_CONV_BOTTLENECK) launches the fused Bottleneck of ops i .. i + 2
+  std::vector<char> fused;             // op i is a later conv of a fused block or Bottleneck: no launch of its own
   int n_launches = 0;
   int batch = 0, act_dtype = 0, n_streams = 1;
   char* arena = nullptr;
@@ -221,17 +222,18 @@ struct acr_b200_plan {
   cudaEvent_t ev_begin = nullptr;
 };
 
-// Fused BasicBlocks (ACR_CONV_BLOCK) are on by default; ACR_B200_FUSE_BLOCKS=0 (read at plan creation) launches the two
-// convs of every block separately again (A/B timing).
+// Fused BasicBlocks (ACR_CONV_BLOCK) and Bottlenecks (ACR_CONV_BOTTLENECK) are on by default; ACR_B200_FUSE_BLOCKS=0
+// (read at plan creation) launches the convs of every block separately again (A/B timing).
 static bool fuse_blocks_enabled() {
   const char* e = getenv("ACR_B200_FUSE_BLOCKS");
   return !(e && atoi(e) == 0);
 }
 
-// the launch of op i: nothing for the second conv of a fused block, the fused kernel for its first
+// the launch of op i: nothing for the later convs of a fused block or Bottleneck, the fused kernel for its first
 static int launch_op(acr_b200_plan* p, int i, const void* image, cudaStream_t st) {
   if (p->fused[i]) return ACR_B200_OK;
   if (p->blk[i]) return conv_block_launch(p->blk[i], st);
+  if (p->bnk[i]) return conv_bottleneck_launch(p->bnk[i], st);
   return run_one(p->ops[i], p->batch, p->arena, p->weights, static_cast<const char*>(image), p->act_dtype, p->tc[i], st);
 }
 
@@ -246,6 +248,7 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
   p->ops.assign(ops, ops + n_ops);
   p->tc.assign(n_ops, nullptr);
   p->blk.assign(n_ops, nullptr);
+  p->bnk.assign(n_ops, nullptr);
   p->fused.assign(n_ops, 0);
   p->batch = batch; p->act_dtype = act_dtype;
   p->arena = static_cast<char*>(arena); p->arena_bytes = arena_bytes;
@@ -263,7 +266,27 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
       if (need > arena_bytes) { set_error("op %d: output exceeds the arena (%zu > %zu)", i, need, arena_bytes); rc = ACR_B200_EINVAL; break; }
     }
     if (p->fused[i]) continue;
-    const bool tc_conv = op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32;   // (the TF32 plan ignores ACR_CONV_BLOCK)
+    const bool tc_conv = op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32;   // (the TF32 plan ignores the fusion flags)
+    if (tc_conv && act_dtype != ACR_DT_TF32 && (op.shift[0] & ACR_CONV_BOTTLENECK) && fuse_blocks_enabled()) {
+      // one launch for the Bottleneck of ops i .. i + 2 (the engine marks only such triples); the later ops' waits must be
+      // ones op i already has
+      bool ok = i + 2 < n_ops;
+      for (int j = i + 1; ok && j <= i + 2; ++j)
+        ok = p->ops[j].kind == ACR_OP_CONV && p->ops[j].stream_id == op.stream_id &&
+             (p->ops[j].wait_mask & ~op.wait_mask & ~(1 << op.stream_id)) == 0;
+      if (!ok) {
+        set_error("op %d: ACR_CONV_BOTTLENECK needs the block's other two convs next, on the same stream", i);
+        rc = ACR_B200_EINVAL;
+        break;
+      }
+      ConvArgs a1, a2, a3;
+      rc = make_conv_args(op, batch, p->arena, p->weights, nullptr, &a1);
+      if (rc == ACR_B200_OK) rc = make_conv_args(p->ops[i + 1], batch, p->arena, p->weights, nullptr, &a2);
+      if (rc == ACR_B200_OK) rc = make_conv_args(p->ops[i + 2], batch, p->arena, p->weights, nullptr, &a3);
+      if (rc == ACR_B200_OK) rc = conv_bottleneck_prepare(a1, a2, a3, act_dtype, &p->bnk[i]);
+      p->fused[i + 1] = p->fused[i + 2] = 1;
+      continue;
+    }
     if (tc_conv && act_dtype != ACR_DT_TF32 && (op.shift[0] & ACR_CONV_BLOCK) && fuse_blocks_enabled()) {
       // one launch for the BasicBlock of ops i and i + 1 (the engine marks only such pairs); op i + 1's waits must be
       // ones op i already has, so nothing that op i + 1 waited for can be missed
@@ -350,8 +373,8 @@ extern "C" int acr_b200_plan_run(acr_b200_plan* p, const void* image, void* stre
   return ACR_B200_OK;
 }
 
-// one serialised pass with an event after every op: device milliseconds of op i into ms_by_op[i] (a fused block's time
-// is on its first conv, its second conv reads 0)
+// one serialised pass with an event after every op: device milliseconds of op i into ms_by_op[i] (a fused block's or
+// Bottleneck's time is on its first conv, its later convs read 0)
 static int profile_ops(acr_b200_plan* p, const void* image, cudaStream_t st, float* ms_by_op) {
   const int n = (int)p->ops.size();
   std::vector<cudaEvent_t> ev(n + 1);
@@ -409,6 +432,7 @@ extern "C" void acr_b200_plan_destroy(acr_b200_plan* p) {
   if (!p) return;
   for (ConvTcPlan* t : p->tc) conv_tc_free(t);
   for (ConvBlockPlan* b : p->blk) conv_block_free(b);
+  for (ConvBottleneckPlan* b : p->bnk) conv_bottleneck_free(b);
   for (int s = 1; s < MAX_STREAMS; ++s)
     if (p->streams[s]) cudaStreamDestroy(p->streams[s]);
   for (cudaEvent_t e : p->ev_op)

@@ -304,7 +304,7 @@ enum {
   ACR_OP_MAXPOOL = 12      /* nn.MaxPool2d(3, stride 2, padding 1) on 16-bit NHWC (ResNet trunk)                     */
 };  /* kinds stay below 16: acr_b200_plan_profile indexes ms_by_kind[16] */
 enum { ACR_CONV_BIAS_PER_IMAGE = 1, ACR_CONV_POW11_CH0 = 2, ACR_CONV_XPAIR = 4, ACR_CONV_S2X = 8, ACR_CONV_EXTRA = 16,
-       ACR_CONV_DECONV = 32, ACR_CONV_BLOCK = 64, ACR_CONV_BLOCK_MID = 128 };
+       ACR_CONV_DECONV = 32, ACR_CONV_BLOCK = 64, ACR_CONV_BLOCK_MID = 128, ACR_CONV_BOTTLENECK = 256 };
 enum { ACR_DT_BF16 = 0, ACR_DT_F16 = 1, ACR_DT_F32 = 2, ACR_DT_U8 = 3,
        ACR_DT_TF32 = 4 /* an act_dtype only (plan_create, run_op, pack_conv): fp32 storage, tf32 tensor-core convs */ };
 
@@ -355,6 +355,13 @@ typedef struct acr_b200_tensor {  /* NHWC activation inside the arena (per-image
             (csrc/conv_block.cuh); bit-identical to two launches.  ACR_B200_FUSE_BLOCKS=0 in the environment at plan
             creation ignores the flag)  | ACR_CONV_BLOCK_MID (with ACR_CONV_BLOCK: the fused launch still writes this
             op's output, for readers outside the plan)
+            | ACR_CONV_BOTTLENECK (this conv and the NEXT TWO ops are one Bottleneck: this op a 1x1 stride-1 C_in -> 64 conv
+            with ReLU, C_in = 64 or 256; the next a 3x3 stride-1 64 -> 64 conv with ReLU on this op's output; the one after
+            a 1x1 stride-1 64 -> 256 conv with ReLU on that output, whose residual is any 256-channel tensor of the same
+            grid (the block input, or the downsample's output).  Both intermediates have no reader outside the triple and
+            are not written.  The three ops sit on one stream, and the second and third wait for nothing this op does
+            not.  The plan runs the triple as ONE launch (csrc/conv_bottleneck.cuh); bit-identical to three launches.
+            ACR_B200_FUSE_BLOCKS=0 at plan creation ignores this flag too)
             Contracts of the tensor-core CONV: k in {1, 3} (4 with ACR_CONV_DECONV), stride in {1, 2}; a 1x1
  *            stride-2 conv (ResNet downsample, padding 0) reads input pixel (2y, 2x); cin_pad and cout_pad are
  *            multiples of 16 up to 2048 (K per tap up to 2048, N up to 2048 as 16 balanced virtual tiles of 128).
@@ -398,8 +405,8 @@ typedef struct acr_b200_plan acr_b200_plan;
  *                             come from acr_b200_pack_conv(..., ACR_DT_TF32); the kernel rounds activations to the nearest
  *                             tf32 in shared memory (storage stays fp32).  Every other
  *                             op (stem, fuse, bilinear, coord, pooling, CONV_REF) runs on the validation plan's kernels,
- *                             the part head as in every plan.  ACR_CONV_BLOCK marks are ignored (two resident fp32 weight
- *                             sets do not fit the fused BasicBlock's shared memory), and the x-paired, stride-2 x-paired
+ *                             the part head as in every plan.  ACR_CONV_BLOCK and ACR_CONV_BOTTLENECK marks are ignored (the
+ *                             resident fp32 weight sets do not fit the fused kernels' shared memory), and the x-paired, stride-2 x-paired
  *                             and transposed conv forms are ACR_B200_EINVAL.
  * A tensor record whose dtype is ACR_DT_TF32 is ACR_B200_EINVAL (here and in acr_b200_run_op).                           */
 int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch, void* arena,
@@ -413,14 +420,15 @@ int acr_b200_plan_run(acr_b200_plan* plan, const void* image, void* stream);
 int acr_b200_plan_profile(acr_b200_plan* plan, const void* image, void* stream, float* ms_by_kind,
                           int32_t* n_by_kind);
 /* The same serialised, event-bracketed pass, but writes the device milliseconds of op i into ms_by_op[i]
- * (host array of n_ops floats, in plan order; a fused BasicBlock's time is on its first conv, the second reads 0).
+ * (host array of n_ops floats, in plan order; a fused BasicBlock's or Bottleneck's time is on its first conv, the others
+ * read 0).
  * Synchronises `stream`.  Per-layer tables.                                                 */
 int acr_b200_plan_profile_ops(acr_b200_plan* plan, const void* image, void* stream, float* ms_by_op);
 /* Number of kernel launches one plan_run issues (for bench.py's gpu_launches): the plan's ops less the
- * second convs of fused BasicBlocks (ACR_CONV_BLOCK).                                       */
+ * second convs of fused BasicBlocks (ACR_CONV_BLOCK) and the second and third of fused Bottlenecks (ACR_CONV_BOTTLENECK). */
 int acr_b200_plan_num_launches(const acr_b200_plan* plan);
 /* launch_of_op[i] (host array of n_ops int32) = index of the launch that computes op i: the two convs of a fused
- * BasicBlock share one launch.                                                              */
+ * BasicBlock, and the three of a fused Bottleneck, share one launch.                                                              */
 int acr_b200_plan_op_launch(const acr_b200_plan* plan, int32_t* launch_of_op);
 void acr_b200_plan_destroy(acr_b200_plan* plan);
 

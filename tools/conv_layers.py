@@ -56,17 +56,33 @@ class ClockSampler(threading.Thread):
         return float(np.median(self.mhz)) if self.mhz else None
 
 
-def conv_classes(recs, batch, blocks=()):
+def conv_classes(recs, batch, blocks=(), bottlenecks=()):
     """[(key, [rec indices], GFLOP, algorithmic MB, weights KB, issued GFLOP)] of the conv launches, in plan order of first
     use.  `blocks`: first records of the BasicBlocks that run as one fused launch (csrc/conv_block.cuh), a class of their
     own (k "3+3"): FLOP of both convs, bytes in + out, and the issued FLOP of the fused kernel (conv1 runs 8 M blocks of 64
-    flat rows per 16x16 tile, 2x its pixels; the x-paired form issues its side taps at full width, 4/3)."""
+    flat rows per 16x16 tile, 2x its pixels; the x-paired form issues its side taps at full width, 4/3).
+    `bottlenecks`: first records of the Bottlenecks that run as one fused launch (csrc/conv_bottleneck.cuh), a class of
+    their own (k "1+3+1", cin = the block input's channels): FLOP of the three convs, bytes in + residual (when it is not
+    the input) + out, and the issued FLOP (conv1 runs 8 M blocks of 64 flat rows per 16x16 tile, 2x its pixels)."""
     agg = collections.OrderedDict()
-    blocks = set(blocks)
+    blocks, bottlenecks = set(blocks), set(bottlenecks)
     for i, r in enumerate(recs):
-        if r["kind"] != L.OP_CONV or i - 1 in blocks:
+        if r["kind"] != L.OP_CONV or i - 1 in blocks or i - 1 in bottlenecks or i - 2 in bottlenecks:
             continue
         x, y, at = r["ins"][0], r["out"], r["attrs"]
+        if i in bottlenecks:
+            r3 = recs[i + 2]
+            mid, out, res = y.C, r3["out"], r3["ins"][1]
+            key = (x.C, out.C, "1+3+1", 1, x.H, True)
+            a = agg.setdefault(key, [[], 0.0, 0.0, 0.0, 0.0])
+            a[0] += [i, i + 1, i + 2]
+            px = out.H * out.W * batch
+            f1, f2, f3 = (2.0 * px * c / 1e9 for c in (mid * x.C, mid * mid * 9, out.C * mid))
+            a[1] += f1 + f2 + f3
+            a[2] += px * (x.C + out.C + (res.C if res is not x else 0)) * 2 / 1e6
+            a[3] = (mid * x.C + mid * mid * 9 + out.C * mid) * 2 / 1024
+            a[4] += 2 * f1 + f2 + f3
+            continue
         if i in blocks:
             key = (x.C, y.C, "3+3", 1, x.H, True)
             a = agg.setdefault(key, [[], 0.0, 0.0, 0.0, 0.0])
@@ -108,7 +124,8 @@ def main():
     ms_op = None
     if args.dry_run:
         eng = Engine(None, args.batch, "cpu", dry_run=True, backbone=args.backbone)
-        blocks = eng.block_starts if os.environ.get("ACR_B200_FUSE_BLOCKS", "1") != "0" else []
+        fuse = os.environ.get("ACR_B200_FUSE_BLOCKS", "1") != "0"
+        blocks, bottlenecks = (eng.block_starts, eng.bottleneck_starts) if fuse else ([], [])
         mhz = args.sm_mhz or 1600.0
         print(f"dry run (no GPU): batch {args.batch}, floors at {args.sms} SMs x {mhz:.0f} MHz and {args.hbm_gbs:.0f} GB/s")
     else:
@@ -133,6 +150,7 @@ def main():
         ms_op = np.median(runs, axis=0)
         launch = eng.launch_of_rec()
         blocks = [i for i in eng.block_starts if launch[i] == launch[i + 1]]
+        bottlenecks = [i for i in eng.bottleneck_starts if launch[i] == launch[i + 2]]
         mhz = args.sm_mhz or sampled or 1600.0
         print(f"{name}, power limit {plimit} W, SM clock {sampled if sampled else 'n/a'} MHz (median during the passes); "
               f"batch {args.batch}, median of {args.passes} passes after {args.warmup} warm-up; "
@@ -140,10 +158,10 @@ def main():
 
     peak_tflops = args.sms * FLOP_PER_CLK_SM * mhz * 1e6 / 1e12
     rows = []
-    for key, idx, gflop, mb, wkb, issued in conv_classes(eng.recs, args.batch, blocks):
+    for key, idx, gflop, mb, wkb, issued in conv_classes(eng.recs, args.batch, blocks, bottlenecks):
         t_c, t_m = issued / peak_tflops, mb / args.hbm_gbs       # ms (compute floor: the FLOP the kernel issues)
         ms = float(ms_op[idx].sum()) if ms_op is not None else None
-        rows.append((key, len(idx) // (2 if key[2] == "3+3" else 1), wkb, gflop, mb, t_c, t_m, ms))   # launches
+        rows.append((key, len(idx) // {"3+3": 2, "1+3+1": 3}.get(key[2], 1), wkb, gflop, mb, t_c, t_m, ms))   # launches
     rows.sort(key=lambda r: -(r[7] if r[7] is not None else max(r[5], r[6])))
     head = "| cin | cout | k | s | H_in | res | n | weights KB | GFLOP | MB | compute floor ms | HBM floor ms | bound |"
     if ms_op is not None:
@@ -157,7 +175,7 @@ def main():
         print(line)
     tc, tm = sum(r[5] for r in rows), sum(r[6] for r in rows)
     tf = sum(max(r[5], r[6]) for r in rows)
-    tail = (f"\n{sum(r[1] for r in rows)} conv launches ({len(blocks)} fused blocks), {sum(r[3] for r in rows):.0f} GFLOP, {sum(r[4] for r in rows) / 1e3:.1f} GB; "
+    tail = (f"\n{sum(r[1] for r in rows)} conv launches ({len(blocks)} fused blocks, {len(bottlenecks)} fused Bottlenecks), {sum(r[3] for r in rows):.0f} GFLOP, {sum(r[4] for r in rows) / 1e3:.1f} GB; "
             f"floors: compute {tc:.1f} ms, HBM {tm:.1f} ms, sum of per-class max {tf:.1f} ms")
     if ms_op is not None:
         t = sum(r[7] for r in rows)
