@@ -229,6 +229,42 @@ class Engine:
                                             cout_pad, cin_pad, self.plan_dt, wp.ctypes.data, bias.ctypes.data), "pack_conv")
         return blob.add(wp)
 
+    def _pack_stem(self, sd, blob: _Blob, wkey: str, bnkey: str, kch: int) -> Tuple[int, int]:
+        """Stem conv (64,3,k,k) OIHW + BN as a (64, kch, 1, 1) GEMM with input channel (ky*k+kx)*3+ci (BN folded by
+        pack_conv): kch = 32 for the 3x3 stem (27 taps), 160 for the 7x7 one (147 taps)."""
+        w = np.ascontiguousarray(sd[wkey + ".weight"], np.float32)
+        ks = w.shape[-1]
+        w1 = np.zeros((64, kch, 1, 1), np.float32)
+        w1[:, :3 * ks * ks, 0, 0] = w.transpose(0, 2, 3, 1).reshape(64, 3 * ks * ks)
+        sd_stem = {"stem.weight": w1}
+        for nme in ("weight", "bias", "running_mean", "running_var"):
+            sd_stem[f"stembn.{nme}"] = np.ascontiguousarray(sd[f"{bnkey}.{nme}"], np.float32)
+        return self._pack_conv(sd_stem, blob, "stem", "stembn", False, kch, 64)
+
+    def _pack_merged(self, sd, blob: _Blob, wkeys, bnkeys, has_bias: bool, k: int, cin_pad: int, each: int) -> Tuple[int, int]:
+        """Convs of identical geometry on the same input as one wide conv: weights / biases concatenated along cout."""
+        wps, bs = [], []
+        for wk, bk in zip(wkeys, bnkeys):
+            tmp = _Blob()
+            self._pack_conv(sd, tmp, wk, bk, has_bias, cin_pad, each)
+            raw = tmp.tobytes()
+            nw = each * k * k * cin_pad * np.dtype(self.npw).itemsize
+            wps.append(np.frombuffer(raw[:nw], self.npw))
+            boff = _rup(nw, 256)
+            bs.append(np.frombuffer(raw[boff: boff + each * 4], np.float32))
+        return blob.add(np.concatenate(wps)), blob.add(np.concatenate(bs))
+
+    @staticmethod
+    def fold_weights(sd, side: str) -> np.ndarray:
+        """contact_layers[4|5] (109, 218) folded onto the 128-wide head tensor: out = W[:, :109].pm + W[:, 109:112].pm[:3]
+        + (b + W[:, 112:].pare), pm = [cam3 | params106] (acr/model.py:158-164); input channel order of the 128-wide
+        tensor: params at 0..105, cam at 112..114.  -> (109, 128, 1, 1) fp32."""
+        W = np.ascontiguousarray(sd[f"contact_layers.{4 if side == 'l' else 5}.weight"], np.float32).reshape(109, 218)
+        weff = np.zeros((109, 128, 1, 1), np.float32)
+        weff[:, :106, 0, 0] = W[:, 3:109]
+        weff[:, 112:115, 0, 0] = W[:, 0:3] + W[:, 109:112]
+        return weff
+
     # --------------------------------------------------------------------- plan
     def _build(self, sd, reuse_memory: bool, shared_weights: Optional[torch.Tensor] = None) -> None:
         spec, B = self.spec, self.batch
@@ -475,24 +511,11 @@ class Engine:
                     o.w_offset[0], o.w_offset[1] = self._pack_deconv(sd, blob, a["w"], a["bn"], o.cin_pad, o.cout_pad)
                     o.shift[0] |= L.CONV_DECONV
                 elif "stem" in a:
-                    # weights (64,3,3,3) OIHW -> (64, 32, 1, 1) with input channel (ky*3+kx)*3+ci; BN folded by pack_conv
-                    w = f32(a["stem"]["w"] + ".weight")
-                    w1 = np.zeros((64, 32, 1, 1), np.float32)
-                    w1[:, :27, 0, 0] = w.transpose(0, 2, 3, 1).reshape(64, 27)
-                    sd_stem = {"stem.weight": w1}
-                    for nme in ("weight", "bias", "running_mean", "running_var"):
-                        sd_stem[f"stembn.{nme}"] = f32(f"{a['stem']['bn']}.{nme}")
                     o.cin_pad, o.cout_pad = 32, 64
-                    o.w_offset[0], o.w_offset[1] = self._pack_conv(sd_stem, blob, "stem", "stembn", False, 32, 64)
+                    o.w_offset[0], o.w_offset[1] = self._pack_stem(sd, blob, a["stem"]["w"], a["stem"]["bn"], 32)
                 elif "fold_side" in a:
-                    # out = W[:, :109].pm + W[:, 109:112].pm[:3] + (b + W[:, 112:].pare),  pm = [cam3 | params106]
-                    # (acr/model.py:158-164); input channel order of the 128-wide tensor: params at 0..105, cam at 112..114
-                    W = f32(f"contact_layers.{4 if a['fold_side'] == 'l' else 5}.weight").reshape(109, 218)
-                    weff = np.zeros((109, 128, 1, 1), np.float32)
-                    weff[:, :106, 0, 0] = W[:, 3:109]
-                    weff[:, 112:115, 0, 0] = W[:, 0:3] + W[:, 109:112]
                     o.cin_pad = 128
-                    o.w_offset[0] = self._pack_raw(blob, weff, o.cin_pad, o.cout_pad)
+                    o.w_offset[0] = self._pack_raw(blob, self.fold_weights(sd, a["fold_side"]), o.cin_pad, o.cout_pad)
                     o.shift[0] |= 1     # ACR_CONV_BIAS_PER_IMAGE (aux[0] = bias_img from the part head)
                 elif s2x:
                     o.cin_pad = 64
@@ -503,19 +526,8 @@ class Engine:
                     o.w_offset[0], o.w_offset[1] = self._pack_conv(sd, blob, a["w"], a["bn"], a["bias"], 64, 64, pair=True)
                     o.shift[0] |= 4     # ACR_CONV_XPAIR: side taps are 32x32 corners of the 64x64 block
                 elif a.get("merged"):
-                    # convs of identical geometry on the same input: weights / biases concatenated along cout
-                    each = a["merged"]
-                    wps, bs = [], []
-                    for wk, bk in zip(a["w"], a["bn"]):
-                        tmp = _Blob()
-                        self._pack_conv(sd, tmp, wk, bk, a["bias"], o.cin_pad, each)
-                        raw = tmp.tobytes()
-                        nw = each * a["k"] * a["k"] * o.cin_pad * np.dtype(self.npw).itemsize
-                        wps.append(np.frombuffer(raw[:nw], self.npw))
-                        boff = _rup(nw, 256)
-                        bs.append(np.frombuffer(raw[boff: boff + each * 4], np.float32))
-                    o.w_offset[0] = blob.add(np.concatenate(wps))
-                    o.w_offset[1] = blob.add(np.concatenate(bs))
+                    o.w_offset[0], o.w_offset[1] = self._pack_merged(sd, blob, a["w"], a["bn"], a["bias"], a["k"], o.cin_pad,
+                                                                     a["merged"])
                 else:
                     o.w_offset[0], o.w_offset[1] = self._pack_conv(sd, blob, a["w"], a["bn"], a["bias"], o.cin_pad, o.cout_pad)
                     if a.get("pow11"):
@@ -525,18 +537,9 @@ class Engine:
                 if r.get("bottleneck"):
                     o.shift[0] |= L.CONV_BOTTLENECK
             elif r["kind"] == L.OP_STEM_TC:
-                # weights (64,3,k,k) OIHW -> (64, K, 1, 1) with input channel (ky*k+kx)*3+ci, K = 32 (3x3) or 160 (7x7: k = 7
-                # in the op); BN folded by pack_conv
-                w = f32(a["stem"]["w"] + ".weight")
-                ks = w.shape[-1]
-                kch = 32 if ks == 3 else 160
-                w1 = np.zeros((64, kch, 1, 1), np.float32)
-                w1[:, :3 * ks * ks, 0, 0] = w.transpose(0, 2, 3, 1).reshape(64, 3 * ks * ks)
-                sd_stem = {"stem.weight": w1}
-                for nme in ("weight", "bias", "running_mean", "running_var"):
-                    sd_stem[f"stembn.{nme}"] = f32(f"{a['stem']['bn']}.{nme}")
-                o.w_offset[0], o.w_offset[1] = self._pack_conv(sd_stem, blob, "stem", "stembn", False, kch, 64)
-                if ks == 7:
+                ks = sd[a["stem"]["w"] + ".weight"].shape[-1]
+                o.w_offset[0], o.w_offset[1] = self._pack_stem(sd, blob, a["stem"]["w"], a["stem"]["bn"], 32 if ks == 3 else 160)
+                if ks == 7:   # k = 7 in the op
                     o.k = 7
             elif r["kind"] == L.OP_STEM:
                 w = f32(a["w"] + ".weight")                                   # (64,3,3,3) OIHW

@@ -58,19 +58,25 @@ CONV_BIAS_PER_IMAGE, CONV_POW11_CH0 = 1, 2     # ACR_CONV_* flag bits (shift[0])
 
 
 def run_conv_case(kind, B, H, W, cin, cout, k, s, relu, residual, bias, bn, out_f32, dt=L.DT_BF16, seed=0,
-                  in_stride=None, cin_pad=None, flags=0, bias_img=None):
-    """Runs one conv through acr_b200_run_op on the GPU and returns (got, expected) fp32 NCHW.
+                  in_stride=None, cin_pad=None, flags=0, bias_img=None, ch_scale=False, bound=False):
+    """Runs one conv through acr_b200_run_op on the GPU and returns (got, expected, pad_ok), fp32 NCHW got and fp64
+    expected, plus the accumulation bound acc of tests.pack_ref.conv_with_bound when ``bound``.
 
+    The expected output is computed in fp64 on the rounded input and on the restated rounding of the ORIGINAL weights
+    (tests/pack_ref.py, pinned to the packer bit for bit by tests/test_cpu_packing.py), in the kernel's epilogue order:
+    + bias, 1.1 ** channel 0, + residual, ReLU.
     flags: ACR_CONV_* bits of the op.  With CONV_BIAS_PER_IMAGE the bias is ``bias_img``, an fp32 (B, cout_pad) tensor
-    placed in the arena as aux[0] (the folded part-head conv).  With any flag the expected output is computed in fp64 on
-    the same rounded operands, in the kernel's epilogue order: + bias, 1.1 ** channel 0, + residual, ReLU."""
-    import torch.nn.functional as Fn
+    placed in the arena as aux[0] (the folded part-head conv).  ``ch_scale`` multiplies input channel c by a power of
+    two from 2^-6 (c = 0) to 2^6 (c = cin - 1), so that small channels matter to the bound."""
+    from tests import pack_ref
     g = torch.Generator().manual_seed(seed)
     tdt = torch.bfloat16 if dt == L.DT_BF16 else torch.float16
     in_stride = in_stride or rup(cin, 16)
     cin_pad, cout_pad = cin_pad or rup(cin, 16), rup(cout, 16)
     Ho, Wo = H // s, W // s
     x = torch.randn(B, cin, H, W, generator=g)
+    if ch_scale:
+        x = x * torch.exp2(torch.round(torch.linspace(-6, 6, cin))).view(1, cin, 1, 1)
     w = torch.randn(cout, cin, k, k, generator=g) * (2.0 / (cin * k * k)) ** 0.5
     cb = torch.randn(cout, generator=g) * 0.1 if bias else None
     bnp = None
@@ -127,18 +133,13 @@ def run_conv_case(kind, B, H, W, cin, cout, k, s, relu, residual, bias, bn, out_
     got = raw.view(torch.float32 if out_f32 else tdt).view(B, Ho, Wo, cout_pad).float()
     pad_ok = bool((got[..., cout:] == 0).all())
     got = got[..., :cout].permute(0, 3, 1, 2).contiguous()
-    # expected: same rounded operands, fp32 math on the CPU (fp64 with flags)
-    wf = u16_to_float(wp, dt).view(cout_pad, k, k, cin_pad)[:cout, :, :, :cin].permute(0, 3, 1, 2).contiguous()
+    # expected: the restated weights (not the packer's words) and the same rounded activations, fp64 on the CPU
+    wq, bq = pack_ref.pack_conv_ref(w.numpy(), None if cb is None else cb.numpy(),
+                                    None if bnp is None else [t.numpy() for t in bnp], dt)
+    wf = torch.from_numpy(pack_ref.words_to_f64(wq, dt))
     xf = xin[..., :cin].float().permute(0, 3, 1, 2).contiguous()
-    if flags:
-        exp = Fn.conv2d(xf.double(), wf.double(), None, s, k // 2)
-        exp = exp + (bias_img[:, :cout, None, None] if per_image else torch.from_numpy(bvec[:cout].copy()).view(1, -1, 1, 1)).double()
-        if flags & CONV_POW11_CH0:
-            exp = torch.cat([torch.pow(1.1, exp[:, :1]), exp[:, 1:]], 1)
-    else:
-        exp = Fn.conv2d(xf, wf, torch.from_numpy(bvec[:cout].copy()), s, k // 2)
-    if residual:
-        exp = exp + rin[..., :cout].float().permute(0, 3, 1, 2)
-    if relu:
-        exp = torch.relu(exp)
-    return got, exp, pad_ok
+    rf = rin[..., :cout].float().permute(0, 3, 1, 2) if residual else None
+    bf = bias_img[:, :cout, None, None] if per_image else torch.from_numpy(bq)
+    exp, acc = pack_ref.conv_with_bound(xf, wf, bf, s, pack_ref.U_ACC_TC, residual=rf,
+                                        pow11=bool(flags & CONV_POW11_CH0), relu=relu)
+    return (got, exp, pad_ok, acc) if bound else (got, exp, pad_ok)

@@ -33,24 +33,46 @@ CASES = [
 ]
 
 
+# more inputs for the same checks: a 13th element holds run_conv_case keywords (and "dt" to override the test's dtype)
+EXTRA_CASES = [
+    (1, 32, 32, 64, 48, 3, 1, True, False, False, True, False),     # N tails: cout_pad not a multiple of 128
+    (1, 32, 32, 64, 112, 1, 1, True, False, True, True, False),
+    (1, 32, 32, 64, 144, 3, 1, True, True, False, True, False),
+    (1, 16, 16, 128, 400, 1, 1, False, False, True, False, False),
+    (1, 32, 32, 48, 64, 3, 1, True, False, False, True, False, (("in_stride", 48), ("cin_pad", 64))),     # K tails
+    (1, 32, 32, 96, 96, 3, 2, True, False, False, True, False, (("in_stride", 96), ("cin_pad", 128))),
+    (2, 32, 32, 64, 64, 3, 1, True, True, False, True, False, (("ch_scale", True),)),   # channels 2^-6 .. 2^6
+    (1, 32, 32, 128, 144, 1, 1, False, False, True, False, False, (("ch_scale", True),)),
+    (1, 64, 64, 48, 109, 1, 1, False, False, True, False, True, (("ch_scale", True), ("in_stride", 48), ("cin_pad", 64))),
+]
+
+
 def _check(kind, case, dt=L.DT_BF16):
-    B, H, W, cin, cout, k, s, relu, res, bias, bn, f32 = case
-    got, exp, pad_ok = run_conv_case(kind, B, H, W, cin, cout, k, s, relu, res, bias, bn, f32, dt=dt,
-                                     seed=hash(case) % 1000)
-    scale = exp.abs().max().item()
-    err = (got - exp).abs().max().item()
-    # fp32 accumulate on identical operands: only summation order + one output rounding differ
-    tol = scale * (2e-5 if f32 else (2 ** -8 if dt == L.DT_BF16 else 2 ** -10)) + 1e-6
+    """Every output element within the fp64 bound of tests/pack_ref.py (exact conv of the rounded operands; accumulation
+    bound; one rounding to the output type), and 16-bit outputs whose rounding the bound decides rounded to nearest
+    (tests.pack_ref.direction_counts)."""
+    from tests.pack_ref import check_bound, direction_counts, direction_ok
+    B, H, W, cin, cout, k, s, relu, res, bias, bn, f32 = case[:12]
+    kw = dict(case[12]) if len(case) > 12 else {}
+    dt = kw.pop("dt", dt)
+    got, exp, pad_ok, acc = run_conv_case(kind, B, H, W, cin, cout, k, s, relu, res, bias, bn, f32, dt=dt,
+                                          seed=hash(case[:12]) % 1000, bound=True, **kw)
     assert pad_ok, "padding channels of the output are not zero"
-    assert err <= tol, f"max err {err:.4g} > tol {tol:.4g} (scale {scale:.3g})"
+    tdt = torch.float32 if f32 else (torch.bfloat16 if dt == L.DT_BF16 else torch.float16)
+    worst, n_bad = check_bound(got, exp, acc, tdt)
+    (toward, away), (t_all, a_all) = ((0, 0), (0, 0)) if f32 else direction_counts(got, exp, acc, tdt)
+    print(f"conv {case}: worst err/bound {worst:.3f}, off-RNE toward zero / away: decided {toward} / {away}, "
+          f"all {t_all} / {a_all}")
+    assert n_bad == 0, f"{n_bad} elements above their bound (worst err/bound {worst:.3f})"
+    assert direction_ok(toward, away), f"rounding direction: {toward} toward zero vs {away} away"
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", CASES + EXTRA_CASES)
 def test_conv_ref(case):
     _check(L.OP_CONV_REF, case)
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", CASES + EXTRA_CASES)
 def test_conv_tc(case):
     _check(L.OP_CONV, case)
 
@@ -63,7 +85,7 @@ def test_conv_tc_tma_store_epilogue(case, monkeypatch):
     _check(L.OP_CONV, case)
 
 
-@pytest.mark.parametrize("case", CASES[:4])
+@pytest.mark.parametrize("case", CASES + EXTRA_CASES)
 def test_conv_tc_fp16(case):
     _check(L.OP_CONV, case, dt=L.DT_F16)
 

@@ -21,7 +21,7 @@ CASES = [
 ]
 
 
-@pytest.mark.parametrize("case", CASES)
+@pytest.mark.parametrize("case", CASES + [c + ((("dt", L.DT_F16),),) for c in CASES])
 def test_conv_tc_many_tiles_per_cta(case):
     _check(L.OP_CONV, case)
 

@@ -196,7 +196,8 @@ def test_every_op_of_the_resnet_plan_teacher_forced(sd_resnet, dtype):
     """Every launch of the ResNet plan against the oracle on the plan's own stored inputs: the ResNet kinds here, the rest
     (bottleneck convs incl. 1x1 stride 2, heads, SegmNet, pooling, part head) through tests/test_gpu_teacher_forced.sweep."""
     from acr_b200.engine import Engine
-    from tests.test_gpu_teacher_forced import sweep
+    from tests.pack_ref import check_bound, direction_counts, direction_ok
+    from tests.test_gpu_teacher_forced import conv_bound, stem_bound, sweep
     torch.set_num_threads(min(32, os.cpu_count()))
     gi = torch.Generator().manual_seed(123)
     image = torch.randint(0, 256, (1, 512, 512, 3), generator=gi, dtype=torch.uint8)
@@ -210,6 +211,11 @@ def test_every_op_of_the_resnet_plan_teacher_forced(sd_resnet, dtype):
         a = r.get("attrs", {})
         if r["kind"] == L.OP_STEM_TC:
             rows.append((i, "stem 7x7", rel_err(get(r["out"]).numpy(), resnet_ref.stem7(image, sdf).numpy())))
+            g, e64, acc, tdt = stem_bound(eng, i, {k: v.numpy() for k, v in sdf.items()}, eng.weights.cpu().numpy(), image)
+            worst, nbad = check_bound(g, e64, acc, tdt)
+            (tw, aw), (ta, aa) = direction_counts(g, e64, acc, tdt)
+            print(f"stem 7x7: worst err/bound {worst:.3f}, off-RNE toward zero / away: decided {tw} / {aw}, all {ta} / {aa}")
+            assert nbad == 0 and direction_ok(tw, aw), ("stem 7x7", worst, nbad, tw, aw)
         elif r["kind"] == L.OP_MAXPOOL:
             x = eng.view(r["ins"][0])[..., :64].permute(0, 3, 1, 2)
             exp = Fn.max_pool2d(x, 3, 2, 1).permute(0, 2, 3, 1)
@@ -218,6 +224,12 @@ def test_every_op_of_the_resnet_plan_teacher_forced(sd_resnet, dtype):
         elif a.get("deconv"):
             exp = resnet_ref.deconv_bn_relu(get(r["ins"][0]), sdf, a["w"], a["bn"])
             rows.append((i, f"deconv {a['w']}", rel_err(get(r["out"]).numpy(), exp.numpy())))
+            # per element: the live packed weights pinned to the restatement, the fp64 bound and the rounding direction
+            g, e64, acc, tdt = conv_bound(eng, i, {k: v.numpy() for k, v in sdf.items()}, eng.weights.cpu().numpy(), get)
+            worst, nbad = check_bound(g, e64, acc, tdt)
+            (tw, aw), (ta, aa) = direction_counts(g, e64, acc, tdt)
+            print(f"deconv {a['w']}: worst err/bound {worst:.3f}, off-RNE toward zero / away: decided {tw} / {aw}, all {ta} / {aa}")
+            assert nbad == 0 and direction_ok(tw, aw), (a["w"], worst, nbad, tw, aw)
         else:
             rest.append(r)
     kinds = [r["kind"] for r in eng.recs]
