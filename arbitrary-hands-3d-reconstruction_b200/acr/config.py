@@ -25,7 +25,10 @@ _DEFAULTS = dict(
                                                           # HRNet-W48 trunk of BASELINE configs[4] (no reference: parity unpinned)
     input_size=512,                                        # config.py:61
     centermap_size=64, centermap_conf_thresh=0.35,         # config.py:130-131
-    kernel_sizes=[5], max_hand=4,                          # config.py:185,161
+    kernel_sizes=[5], max_hand=4,                          # config.py:185,161 (max_hand is the reference's training-time
+                                                          # value; it does not switch multi-hand parsing on)
+    max_hands_per_side=1,                                  # hands kept per image and side, 1..16; 1 = the reference's
+                                                          # inference parse, > 1 = multi-hand parsing (DESIGN.md)
     Rot_type="6D", rot_dim=6, cam_dim=3, align_idx=9,      # config.py:167-170
     mano_theta_num=16, head_block_num=2,                   # config.py:172,98
     inter_prior=True, prior_mode="cross",                  # config.py:88-89

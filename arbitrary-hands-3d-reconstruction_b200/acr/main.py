@@ -11,6 +11,14 @@ from acr.model import ACR as ACR_v1
 from acr.utils import justify_detection_state, load_model
 
 
+def _check_hands_per_side(K):
+    """A captured graph's parse and MANO launches are sized for the K it was captured with."""
+    from acr.result_parser import ResultParser
+    now = ResultParser.hands_per_side()
+    if now != K:
+        raise ValueError(f"this graph was captured with max_hands_per_side={K}, but it is now {now}: capture it again")
+
+
 class ACR(nn.Module):
     def __init__(self, args_set=None, state_dict=None, mano_assets=None):
         super().__init__()
@@ -34,6 +42,10 @@ class ACR(nn.Module):
         # temporal optimisation (acr/main.py:69-83): OneEuro filters on poses / betas, one bank per hand type,
         # applied between parse and MANO -- here one device kernel instead of host-side filter objects
         if getattr(self, 'temporal_optimization', False):
+            from acr.result_parser import ResultParser
+            if ResultParser.hands_per_side() > 1:
+                raise ValueError("temporal_optimization needs max_hands_per_side=1: the filter banks are per hand type, "
+                                 "and several hands of one side are not tracked across frames")
             from acr_b200 import ops as _ops
             pd = outputs['params_dict']
             assert len(pd['poses']) == 2, 'temporal smoothing streams one frame (two hand slots) at a time'
@@ -60,8 +72,8 @@ class ACR(nn.Module):
     @torch.no_grad()
     def fused_forward(self, images_rgb_u8, offsets, out=None, peers=None):
         """Sync-free pipeline: backbone + heads + parse + MANO enqueued back to back; MANO runs over
-        the worst case 2B rows and skips rows >= L+R on the device.  Returns dense buffers (zero copy: the
-        parse buffers are shared per batch size, consume them before the next call).  ``peers``
+        the worst case 2KB rows (K = ``max_hands_per_side``) and skips rows >= L+R on the device.  Returns dense
+        buffers (zero copy: the parse buffers are shared per batch size, consume them before the next call).  ``peers``
         (acr_b200.dist.PeerVertexGather): the MANO kernel also stores vertices and row counts into every
         rank's gather buffer."""
         B = images_rgb_u8.shape[0]
@@ -82,7 +94,10 @@ class ACR(nn.Module):
         launches) for a fixed batch size: returns ``replay(frames_u8, offsets) -> (bufs, mano)`` that copies
         the inputs into static buffers and launches ONE graph.  This is what makes the reference's
         frame-by-frame video / webcam loop (acr/main.py:183-201, batch 1) latency-bound by the GPU instead
-        of by ~380 host-side launches."""
+        of by ~380 host-side launches.  The graph is bound to the ``max_hands_per_side`` it was captured with
+        (``replay.hands_per_side``); a replay under another value raises."""
+        from acr.result_parser import ResultParser
+        K = ResultParser.hands_per_side()
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         frames = torch.zeros(batch, args().input_size, args().input_size, 3, dtype=torch.uint8, device=dev)
         offsets = torch.zeros(batch, 10, device=dev)
@@ -98,12 +113,13 @@ class ACR(nn.Module):
             bufs, mano = self.fused_forward(frames, offsets)
 
         def replay(frames_u8, offs):
+            _check_hands_per_side(K)
             frames.copy_(frames_u8, non_blocking=True)
             offsets.copy_(offs, non_blocking=True)
             graph.replay()
             return bufs, mano
 
-        replay.graph, replay.static_inputs = graph, (frames, offsets)
+        replay.graph, replay.static_inputs, replay.hands_per_side = graph, (frames, offsets), K
         return replay
 
     @torch.no_grad()
@@ -112,8 +128,11 @@ class ACR(nn.Module):
         white pad, bicubic resize, offsets; acr_b200.preprocess.RaggedFrames) followed by ``fused_forward``.  Returns
         ``replay(frames) -> (bufs, mano)`` for a list of exactly ``batch`` BGR frames (numpy arrays, CPU or CUDA
         tensors) of any sizes, each replay its own, whose packed H*W*3 bytes sum to at most ``max_frame_bytes``.  Host
-        frames travel in one H2D copy; a list that does not fit raises before anything is enqueued."""
+        frames travel in one H2D copy; a list that does not fit raises before anything is enqueued.  Like
+        ``capture_graph``, the graph is bound to its ``max_hands_per_side``."""
+        from acr.result_parser import ResultParser
         from acr_b200.preprocess import RaggedFrames
+        K = ResultParser.hands_per_side()
         import numpy as np
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
@@ -131,11 +150,12 @@ class ACR(nn.Module):
             bufs, mano = self.fused_forward(*rf.launch())
 
         def replay(frames):
+            _check_hands_per_side(K)
             rf.load(frames)
             graph.replay()
             return bufs, mano
 
-        replay.graph, replay.frames = graph, rf
+        replay.graph, replay.frames, replay.hands_per_side = graph, rf, K
         return replay
 
     @torch.no_grad()

@@ -188,7 +188,8 @@ class ACR(nn.Module):
     @torch.no_grad()
     def forward_dense(self, meta_data):
         """Sync-free variant for the fused pipeline: runs backbone + heads + parse and returns the
-        engine and the worst-case (2B rows) parse buffers; row validity lives in ``bufs.counts``.
+        engine and the worst-case (2KB rows, K = ``max_hands_per_side``) parse buffers; row validity lives in
+        ``bufs.counts``.
         ZERO COPY: the returned buffers are the per-batch-size cached ones and alias the next call's
         results -- consume (or copy) them before the next forward of the same batch size."""
         img, dev = self._image(meta_data)

@@ -2,8 +2,8 @@
 
 ``parse(outputs, meta_data, cfg)`` takes the reference's dict of NCHW maps; inside the fused
 pipeline ``parse_engine`` reads the engine's NHWC fp32 maps in place.  Either way the work is three
-small kernels (acr_b200_parse) and exactly one device->host read (the two hand counts) instead
-of the reference's >=6 implicit syncs.
+small kernels (acr_b200_parse, or acr_b200_parse_topk with ``max_hands_per_side`` > 1) and exactly one
+device->host read (the two hand counts) instead of the reference's >=6 implicit syncs.
 """
 from __future__ import annotations
 
@@ -28,19 +28,28 @@ class ResultParser(nn.Module):
                              "(the reference's shipped configuration) are supported")
         self._pbufs = {}
 
-    def _parse_buffers(self, B, device):
-        key = (B, str(device))
+    @staticmethod
+    def hands_per_side():
+        """``args().max_hands_per_side``: hands kept per image and side (1 = the reference's inference parse)."""
+        K = getattr(args(), 'max_hands_per_side', 1)
+        if isinstance(K, bool) or not isinstance(K, int) or not 1 <= K <= _ops.MAX_HANDS_PER_SIDE:
+            raise ValueError(f"max_hands_per_side must be an integer in 1..{_ops.MAX_HANDS_PER_SIDE}, got {K!r}")
+        return K
+
+    def _parse_buffers(self, B, K, device):
+        key = (B, K, str(device))
         if key not in self._pbufs:
-            self._pbufs[key] = _ops.ParseBuffers(B, device)
+            self._pbufs[key] = _ops.ParseBuffers(B, device, K)
         return self._pbufs[key]
 
     # ------------------------------------------------------------------ kernels
     def launch(self, maps, B, meta_data, device):
-        """Enqueue the parse kernels; returns the worst-case buffers (no sync)."""
-        bufs = self._parse_buffers(B, device)
+        """Enqueue the parse kernels; returns the worst-case (2KB rows) buffers (no sync)."""
+        K = self.hands_per_side()
+        bufs = self._parse_buffers(B, K, device)
         ids = meta_data.get('batch_ids') if meta_data is not None else None
         offs = meta_data.get('offsets') if meta_data is not None else None
-        _ops.parse_maps(maps, B, bufs, ids, offs, args().centermap_conf_thresh)
+        _ops.parse_maps(maps, B, bufs, ids, offs, args().centermap_conf_thresh, K)
         return bufs
 
     @staticmethod

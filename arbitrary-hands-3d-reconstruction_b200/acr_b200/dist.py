@@ -42,6 +42,12 @@ def compact_gathered(gathered: torch.Tensor, counts: torch.Tensor) -> List[torch
     return [gathered[r, : int(n[r])] for r in range(gathered.shape[0])]
 
 
+def parse_rows(batch: int, hands_per_side: int = 1) -> int:
+    """Worst-case parse rows of one shard, the ``rows`` a gather buffer needs: 2 * K * batch (K hands per image and
+    side, ``max_hands_per_side``), so always even as PeerVertexGather requires."""
+    return 2 * int(hands_per_side) * int(batch)
+
+
 def gather_layout(world: int, rows: int) -> dict:
     """Byte layout of the symmetric gather allocation (include/acr_b200.h, acr_b200_gather): two slots of
     verts[world][rows][778][3] fp32 + counts[world][8] int32, then flags[world] uint64."""
@@ -63,6 +69,8 @@ class PeerVertexGather:
     s in every rank's flag word.  There is no barrier and no NCCL call: the kernel itself waits (on flags in
     its own memory) until the slot it is about to overwrite has been released, which with two slots is a
     dependency on the PREVIOUS step of the peers.
+
+    ``rows`` is the shard's worst-case parse rows, ``parse_rows(batch, max_hands_per_side)`` = 2KB.
 
     Contract: consume step k's gathered data (``gathered()`` / ``counts()`` after ``finish()``) on the
     launching stream before the next fused launch -- then no peer can overwrite it while it is read.

@@ -263,21 +263,30 @@ def rodrigues(aa: torch.Tensor) -> torch.Tensor:
 
 
 # --------------------------------------------------------------------------------- parse
-class ParseBuffers:
-    """Worst-case (2B rows) output buffers of acr_b200_parse, allocated once per batch size."""
+MAX_HANDS_PER_SIDE = 16
 
-    def __init__(self, B: int, device):
+
+class ParseBuffers:
+    """Worst-case (2KB rows: up to K hands per image and side) output buffers of acr_b200_parse (K = 1) /
+    acr_b200_parse_topk, allocated once per (batch size, K).  ``top_idx`` / ``top_score`` are (B, 2) at K = 1 and
+    (B, 2, K) above."""
+
+    def __init__(self, B: int, device, K: int = 1):
+        if not 1 <= int(K) <= MAX_HANDS_PER_SIDE:
+            raise ValueError(f"hands per side must be in 1..{MAX_HANDS_PER_SIDE}, got {K}")
         f = lambda *s: torch.zeros(*s, device=device, dtype=torch.float32)
         i64 = lambda *s: torch.zeros(*s, device=device, dtype=torch.int64)
         i32 = lambda *s: torch.zeros(*s, device=device, dtype=torch.int32)
-        R = 2 * B
-        self.B = B
+        K = int(K)
+        R = 2 * K * B
+        self.B, self.K = B, K
         self.params_pred, self.cam, self.global_orient = f(R, 109), f(R, 3), f(R, 3)
         self.hand_pose, self.betas, self.poses = f(R, 45), f(R, 10), f(R, 48)
         self.detection_flag, self.reorganize_idx, self.batch_ids = f(R), i64(R), i64(R)
         self.centers_pred, self.centers_conf, self.hand_type = i64(R, 2), f(R), i32(R)
         self.offsets_out, self.counts = f(R, 10), i32(8)
-        self.top_idx, self.top_score, self.row_src = i32(B, 2), f(B, 2), i32(R, 4)
+        top = (B, 2) if K == 1 else (B, 2, K)
+        self.top_idx, self.top_score, self.row_src = i32(*top), f(*top), i32(R, 4)
 
     def struct(self) -> L.ParseOut:
         o = L.ParseOut()
@@ -287,9 +296,13 @@ class ParseBuffers:
 
 
 def parse_maps(maps: Dict[str, tuple], B: int, bufs: ParseBuffers, meta_batch_ids: Optional[torch.Tensor],
-               offsets: Optional[torch.Tensor], conf_thresh: float = 0.35) -> None:
+               offsets: Optional[torch.Tensor], conf_thresh: float = 0.35, K: int = 1) -> None:
     """maps[name] = (fp32 CUDA tensor in NHWC layout, pix_stride) for l/r_center, l/r_params, l/r_prior.
-    Fills ``bufs`` asynchronously on the current stream (no host sync)."""
+    Fills ``bufs`` (built for this B and K) asynchronously on the current stream (no host sync).  K = 1 is the
+    reference's inference parse (acr_b200_parse); K > 1 keeps up to K hands per image and side
+    (acr_b200_parse_topk)."""
+    if bufs.B != B or bufs.K != K:
+        raise ValueError(f"parse buffers are sized for B={bufs.B}, K={bufs.K}, not B={B}, K={K}")
     lib = L.load()
     ms = []
     dev = L.require_cuda(bufs.counts, *[maps[k][0] for k in maps])
@@ -304,8 +317,12 @@ def parse_maps(maps: Dict[str, tuple], B: int, bufs: ParseBuffers, meta_batch_id
     if offsets is not None:
         offsets = offsets.to(device=bufs.counts.device, dtype=torch.float32).contiguous()
     with L.on(dev):
-        rc = lib.acr_b200_parse(*ms, B, float(conf_thresh), L.ptr(meta_batch_ids), L.ptr(offsets), bufs.struct(),
-                                L.current_stream(dev))
+        if K == 1:
+            rc = lib.acr_b200_parse(*ms, B, float(conf_thresh), L.ptr(meta_batch_ids), L.ptr(offsets), bufs.struct(),
+                                    L.current_stream(dev))
+        else:
+            rc = lib.acr_b200_parse_topk(*ms, B, int(K), float(conf_thresh), L.ptr(meta_batch_ids), L.ptr(offsets),
+                                         bufs.struct(), L.current_stream(dev))
     L.check(rc, "parse")
     # keep the inputs alive until the kernels have run
     bufs._keep = (meta_batch_ids, offsets, [m for m in maps.values()])

@@ -13,6 +13,7 @@
 //                   decision, counts.
 //   3. parse_gather grid (2B): per output row gather 109 params at the centre (+106 prior values
 //                   read at the OTHER hand's centre), split, 16 x rot6d->axis-angle.
+// acr_b200_parse_topk (multi-hand, below) keeps up to K hands per image and side with the same gather.
 #include "common.cuh"
 #include "rotation.cuh"
 
@@ -189,6 +190,188 @@ __global__ void __launch_bounds__(128) parse_gather_kernel(ParseParams p) {
     p.o.offsets_out[(size_t)r * 10 + (t - 64)] = p.offsets[(size_t)b * 10 + (t - 64)];
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Multi-hand parsing (acr_b200_parse_topk): up to K hands per image and side, the reference's train_flag=True
+// selection (result_parser.py:218-243 with max_hand = K).  Same three stages as above; the gather stage is
+// parse_gather_kernel itself, launched over 2KB rows.
+//   1. parse_topk      grid (B,2): the NMS of parse_top1, then K block arg-max rounds; each round excludes the
+//                      previous winners.  (score desc, flat index asc) is a total order, so the winners do not
+//                      depend on the reduction order, and round 0 is parse_top1's result bit for bit.
+//   2. parse_topk_scan 1 CTA: hands per image and side (the kept ranks are a prefix), stable compaction "left
+//                      hands image-major / rank-minor, then right hands", dummy rows, the batch-global
+//                      determine_coeff gate on the rank-0 rows, and each hand's prior partner: the nearest
+//                      opposite-side hand of its image (integer squared grid distance, ties to the lower rank).
+constexpr int MAX_HANDS_PER_SIDE = 16;
+constexpr int TOPK_PER_THREAD = NPIX / 256;
+
+struct ParseTopKParams {
+  ParseParams p;  // row_src / top_idx / top_score sized (2KB,4) / (B,2,K)
+  int K;
+};
+
+__device__ __forceinline__ bool topk_before(float v, int i, float bv, int bi) {
+  return v > bv || (v == bv && i < bi);
+}
+
+__global__ void __launch_bounds__(256) parse_topk_kernel(ParseTopKParams q) {
+  __shared__ float s_map[NPIX];
+  __shared__ float s_wv[8];
+  __shared__ int s_wi[8];
+  __shared__ int s_win;
+  const ParseParams& p = q.p;
+  const int K = q.K;
+  const int b = blockIdx.x, side = blockIdx.y, t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const acr_b200_map cm = p.center[side];
+  const float* src = cm.ptr + (size_t)b * NPIX * cm.pix_stride;
+  for (int i = t; i < NPIX; i += 256) s_map[i] = src[(size_t)i * cm.pix_stride];
+  __syncthreads();
+  float sc[TOPK_PER_THREAD];  // NMS scores of pixels t + 256 j
+#pragma unroll
+  for (int j = 0; j < TOPK_PER_THREAD; ++j) {
+    const int i = t + j * 256;
+    const int y = i >> 6, x = i & 63;
+    const float v = s_map[i];
+    float mx = -INFINITY;
+#pragma unroll
+    for (int dy = -2; dy <= 2; ++dy) {
+      const int yy = y + dy;
+      if (yy < 0 || yy >= MAPSZ) continue;
+#pragma unroll
+      for (int dx = -2; dx <= 2; ++dx) {
+        const int xx = x + dx;
+        if (xx < 0 || xx >= MAPSZ) continue;
+        mx = fmaxf(mx, s_map[yy * MAPSZ + xx]);
+      }
+    }
+    sc[j] = (mx == v) ? v : 0.f;  // det * (maxpool(det) == det)
+  }
+  unsigned taken = 0;  // bit j: pixel t + 256 j already selected
+  float bv = -INFINITY;
+  int bi = 0x7fffffff;
+  auto rescan = [&]() {
+    bv = -INFINITY; bi = 0x7fffffff;
+#pragma unroll
+    for (int j = 0; j < TOPK_PER_THREAD; ++j)
+      if (!((taken >> j) & 1u) && topk_before(sc[j], t + j * 256, bv, bi)) { bv = sc[j]; bi = t + j * 256; }
+  };
+  rescan();
+  int32_t* out_idx = p.o.top_idx + (size_t)(b * 2 + side) * K;
+  float* out_score = p.o.top_score + (size_t)(b * 2 + side) * K;
+  for (int k = 0; k < K; ++k) {
+    float v = bv;
+    int i = bi;
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, v, off);
+      const int oi = __shfl_xor_sync(0xffffffffu, i, off);
+      if (topk_before(ov, oi, v, i)) { v = ov; i = oi; }
+    }
+    if (lane == 0) { s_wv[warp] = v; s_wi[warp] = i; }
+    __syncthreads();
+    if (warp == 0) {
+      v = lane < 8 ? s_wv[lane] : -INFINITY;
+      i = lane < 8 ? s_wi[lane] : 0x7fffffff;
+#pragma unroll
+      for (int off = 4; off > 0; off >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, v, off);
+        const int oi = __shfl_xor_sync(0xffffffffu, i, off);
+        if (topk_before(ov, oi, v, i)) { v = ov; i = oi; }
+      }
+      if (lane == 0) { s_win = i; out_idx[k] = i; out_score[k] = v; }
+    }
+    __syncthreads();
+    const int w = s_win;
+    if ((w & 255) == t) {  // the winner's owner drops it and finds its next best
+      taken |= 1u << (w >> 8);
+      rescan();
+    }
+  }
+}
+
+// nearest of the n flat indices `other` to `fi` (integer squared grid distance, ties to the lower rank), or -1
+__device__ __forceinline__ int nearest_partner(int fi, const int32_t* other, int n) {
+  int best = -1, bd = 0x7fffffff;
+  for (int j = 0; j < n; ++j) {
+    const int o = other[j];
+    const int dy = (fi >> 6) - (o >> 6), dx = (fi & 63) - (o & 63);
+    const int d = dy * dy + dx * dx;
+    if (d < bd) { bd = d; best = o; }
+  }
+  return best;
+}
+
+// single CTA of 1024 threads; B is processed in strides of contiguous images per thread
+__global__ void __launch_bounds__(1024, 1) parse_topk_scan_kernel(ParseTopKParams q) {
+  __shared__ int s_cnt[2][1024];
+  __shared__ int s_first[2];
+  const ParseParams& p = q.p;
+  const int t = threadIdx.x, B = p.B, K = q.K;
+  const int per = (B + 1023) / 1024;
+  auto hands = [&](int b, int s) {  // scores are descending, so the kept ranks are a prefix
+    const float* sc = p.o.top_score + (size_t)(b * 2 + s) * K;
+    int n = 0;
+    while (n < K && sc[n] > p.thresh) ++n;
+    return n;
+  };
+  int cl = 0, cr = 0;
+  for (int i = 0; i < per; ++i) {
+    const int b = t * per + i;
+    if (b < B) { cl += hands(b, 0); cr += hands(b, 1); }
+  }
+  s_cnt[0][t] = cl; s_cnt[1][t] = cr;
+  if (t < 2) s_first[t] = 0x7fffffff;
+  __syncthreads();
+  for (int off = 1; off < 1024; off <<= 1) {
+    int a0 = 0, a1 = 0;
+    if (t >= off) { a0 = s_cnt[0][t - off]; a1 = s_cnt[1][t - off]; }
+    __syncthreads();
+    s_cnt[0][t] += a0; s_cnt[1][t] += a1;
+    __syncthreads();
+  }
+  const int nl = s_cnt[0][1023], nr = s_cnt[1][1023];
+  const int L = max(nl, 1), R = max(nr, 1);
+  for (int i = 0; i < per; ++i) {  // first image with a detection of each side (min: order-free)
+    const int b = t * per + i;
+    if (b < B) {
+      if (p.o.top_score[(size_t)(b * 2 + 0) * K] > p.thresh) atomicMin(&s_first[0], b);
+      if (p.o.top_score[(size_t)(b * 2 + 1) * K] > p.thresh) atomicMin(&s_first[1], b);
+    }
+  }
+  __syncthreads();
+  // determine_coeff on the batch's first left and first right rows (rank 0 of their images)
+  bool prior_on = false;
+  if (nl > 0 && nr > 0) {
+    const int il = p.o.top_idx[(size_t)(s_first[0] * 2 + 0) * K], ir = p.o.top_idx[(size_t)(s_first[1] * 2 + 1) * K];
+    const float dy = (float)(il >> 6) - (float)(ir >> 6), dx = (float)(il & 63) - (float)(ir & 63);
+    const float d = sqrtf(dy * dy + dx * dx);
+    prior_on = !(d > 32.f);
+  }
+  int pl = s_cnt[0][t] - cl, pr = s_cnt[1][t] - cr;  // exclusive prefix
+  for (int i = 0; i < per; ++i) {
+    const int b = t * per + i;
+    if (b >= B) break;
+    const int hl = hands(b, 0), hr = hands(b, 1);
+    const int32_t* li = p.o.top_idx + (size_t)(b * 2 + 0) * K;
+    const int32_t* ri = p.o.top_idx + (size_t)(b * 2 + 1) * K;
+    for (int k = 0; k < hl; ++k) {
+      int32_t* r = p.row_src + (size_t)(pl++) * 4;
+      r[0] = b; r[1] = 0; r[2] = li[k];
+      r[3] = prior_on ? nearest_partner(li[k], ri, hr) : -1;
+    }
+    for (int k = 0; k < hr; ++k) {
+      int32_t* r = p.row_src + (size_t)(L + pr++) * 4;
+      r[0] = b; r[1] = 1; r[2] = ri[k];
+      r[3] = prior_on ? nearest_partner(ri[k], li, hl) : -1;
+    }
+  }
+  if (t == 0) {
+    if (nl == 0) { int32_t* r = p.row_src; r[0] = 0; r[1] = 0; r[2] = 0; r[3] = -1; }
+    if (nr == 0) { int32_t* r = p.row_src + (size_t)L * 4; r[0] = 0; r[1] = 1; r[2] = 0; r[3] = -1; }
+    p.o.counts[0] = L; p.o.counts[1] = R; p.o.counts[2] = L + R; p.o.counts[3] = nl + nr;
+    p.o.counts[4] = nl; p.o.counts[5] = nr;
+  }
+}
+
 }  // namespace acr
 
 using namespace acr;
@@ -216,6 +399,36 @@ extern "C" int acr_b200_parse(acr_b200_map l_center, acr_b200_map r_center, acr_
   parse_scan_kernel<<<1, 1024, 0, st>>>(p);
   ACR_CHECK_LAUNCH();
   parse_gather_kernel<<<2 * B, 128, 0, st>>>(p);
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}
+
+extern "C" int acr_b200_parse_topk(acr_b200_map l_center, acr_b200_map r_center, acr_b200_map l_params,
+                                   acr_b200_map r_params, acr_b200_map l_prior, acr_b200_map r_prior, int B, int K,
+                                   float conf_thresh, const int64_t* meta_batch_ids, const float* offsets,
+                                   acr_b200_parse_out out, void* stream) {
+  ACR_CHECK_ARG(B > 0, "parse_topk: B must be positive");
+  ACR_CHECK_ARG(K >= 1 && K <= MAX_HANDS_PER_SIDE, "parse_topk: K must be in 1..16");
+  ACR_CHECK_ARG((long long)B * 2 * K <= 0x7fffffff, "parse_topk: 2*K*B rows overflow");
+  ACR_CHECK_ARG(l_center.ptr && r_center.ptr && l_params.ptr && r_params.ptr && l_prior.ptr && r_prior.ptr,
+                "parse_topk: null map");
+  ACR_CHECK_ARG(out.params_pred && out.cam && out.global_orient && out.hand_pose && out.betas && out.poses &&
+                    out.detection_flag && out.reorganize_idx && out.batch_ids && out.centers_pred &&
+                    out.centers_conf && out.hand_type && out.counts && out.top_idx && out.top_score && out.row_src,
+                "parse_topk: null output buffer");
+  ParseTopKParams q;
+  q.p.center[0] = l_center; q.p.center[1] = r_center;
+  q.p.params[0] = l_params; q.p.params[1] = r_params;
+  q.p.prior[0] = l_prior; q.p.prior[1] = r_prior;
+  q.p.B = B; q.p.thresh = conf_thresh; q.p.meta_ids = meta_batch_ids; q.p.offsets = offsets; q.p.o = out;
+  q.p.row_src = out.row_src;
+  q.K = K;
+  cudaStream_t st = (cudaStream_t)stream;
+  parse_topk_kernel<<<dim3(B, 2), 256, 0, st>>>(q);
+  ACR_CHECK_LAUNCH();
+  parse_topk_scan_kernel<<<1, 1024, 0, st>>>(q);
+  ACR_CHECK_LAUNCH();
+  parse_gather_kernel<<<2 * K * B, 128, 0, st>>>(q.p);
   ACR_CHECK_LAUNCH();
   return ACR_B200_OK;
 }

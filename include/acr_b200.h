@@ -286,6 +286,21 @@ int acr_b200_parse(acr_b200_map l_center, acr_b200_map r_center, acr_b200_map l_
                    float conf_thresh, const int64_t* meta_batch_ids, const float* offsets,
                    acr_b200_parse_out out, void* stream);
 
+/* Multi-hand parsing: up to K hands per image and side, the reference's train_flag=True centre selection
+ * (acr/result_parser.py:218-243 with max_hand = K).  Per image and side: the 5x5 max-pool NMS of acr_b200_parse,
+ * the top K scores in descending order (equal scores: lower flat index first), kept while score > conf_thresh.
+ * Rows: every left hand (image-major, rank-minor), then every right hand; a side with no detection in the batch
+ * gets the dummy row of acr_b200_parse.  The cross-hand prior of hand (b, side, k) is its own side's prior map
+ * sampled at the nearest opposite-side hand of image b (integer squared grid distance, ties to the lower rank),
+ * nothing when image b has none; the batch-global determine_coeff gate uses the first left and first right rows.
+ * K = 1 gives acr_b200_parse's outputs bit for bit.  Capacities: every row buffer of `out` holds 2*K*B rows,
+ * top_idx / top_score are (B,2,K), row_src is (2*K*B,4); counts has the meaning above.
+ * K outside 1..16 is ACR_B200_EINVAL. */
+int acr_b200_parse_topk(acr_b200_map l_center, acr_b200_map r_center, acr_b200_map l_params,
+                        acr_b200_map r_params, acr_b200_map l_prior, acr_b200_map r_prior, int B, int K,
+                        float conf_thresh, const int64_t* meta_batch_ids, const float* offsets,
+                        acr_b200_parse_out out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Network launch plan (backbone + heads)
  * ---------------------------------------------------------------------------------------- */
