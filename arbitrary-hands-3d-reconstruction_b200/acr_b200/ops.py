@@ -228,9 +228,12 @@ def one_euro_smooth(poses: torch.Tensor, betas: torch.Tensor, state: OneEuroStat
                     hand_type: Optional[torch.Tensor] = None, detection_flag: Optional[torch.Tensor] = None,
                     n_dev: Optional[torch.Tensor] = None) -> None:
     """In-place temporal smoothing of (n,48) poses and (n,10) betas (drop-in for acr.utils.smooth_results
-    applied per hand as in acr/main.py:69-83)."""
+    applied per hand as in acr/main.py:69-83).  The state has one bank per hand type, so at most two rows (one per
+    type; row r uses bank r without ``hand_type``): more raise AcrB200Error, like the C entry point."""
     dev = L.require_cuda(poses, betas, hand_type, detection_flag, n_dev, state.state)
     assert poses.is_contiguous() and betas.is_contiguous() and poses.dtype == betas.dtype == torch.float32
+    if poses.shape[0] > 2:
+        raise L.AcrB200Error(f"one_euro_smooth: at most 2 rows, one per hand type (got {poses.shape[0]})")
     if poses.shape[0]:
         with L.on(dev):
             L.check(L.load().acr_b200_one_euro_smooth(L.ptr(poses), L.ptr(betas), L.ptr(hand_type), L.ptr(detection_flag),

@@ -73,6 +73,9 @@ extern "C" int acr_b200_one_euro_smooth(float* poses, float* betas, const int32_
                                         const float* detection_flag, const int32_t* n_dev, int n_max,
                                         float* state, float smooth_coeff, void* stream) {
   ACR_CHECK_ARG(n_max >= 0 && (n_max == 0 || (poses && betas && state)), "one_euro_smooth: bad arguments");
+  // the state has one bank per hand type: a third row would index past it (hand_type NULL: bank = row), or share a
+  // bank with another row's block
+  ACR_CHECK_ARG(n_max <= 2, "one_euro_smooth: at most 2 rows, one per hand type (got %d)", n_max);
   ACR_CHECK_ARG(smooth_coeff > 0.f, "one_euro_smooth: smooth_coeff must be positive");
   if (n_max == 0) return ACR_B200_OK;
   one_euro_kernel<<<n_max, SM_ELEMS, 0, (cudaStream_t)stream>>>(poses, betas, hand_type, detection_flag, n_dev, n_max,

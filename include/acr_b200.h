@@ -232,7 +232,9 @@ int acr_b200_preprocess_ragged(const uint8_t* frames_bgr, int64_t src_bytes, con
  * `state`: device buffer of acr_b200_one_euro_state_floats() floats, zero-initialised = "no history";
  * one filter bank per hand type (0 left, 1 right), like the reference's filter_dict -- i.e. for streaming
  * one frame at a time (the reference asserts exactly two rows).  Rows with detection_flag == 0 are skipped.
- * poses (n,48) and betas (n,10) are updated in place.                                              */
+ * poses (n,48) and betas (n,10) are updated in place.
+ * Row r uses bank hand_type[r], or bank r when hand_type is NULL; the two rows of a call must use different banks.
+ * The state holds two banks, so n_max > 2 is ACR_B200_EINVAL and nothing is launched.                */
 size_t acr_b200_one_euro_state_floats(void);
 int acr_b200_one_euro_smooth(float* poses, float* betas, const int32_t* hand_type, const float* detection_flag,
                              const int32_t* n_dev, int n_max, float* state, float smooth_coeff, void* stream);

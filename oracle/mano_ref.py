@@ -19,6 +19,11 @@ import numpy as np
 from .rotation_ref import batch_rodrigues
 
 F = np.float32
+
+
+def _dtype(dtype):
+    """The type a function computes in: its ``dtype`` argument, or the module's F (float32, the reference's)."""
+    return globals()["F"] if dtype is None else dtype
 LEVELS = ([1, 4, 7, 10, 13], [2, 5, 8, 11, 14], [3, 6, 9, 12, 15])      # manolayer.py:191-193
 CHAIN_REORDER = [0, 1, 6, 11, 2, 7, 12, 3, 8, 13, 4, 9, 14, 5, 10, 15]   # manolayer.py:222
 JOINT_REORDER = [0, 13, 14, 15, 16, 1, 2, 3, 17, 4, 5, 6, 18, 10, 11, 12, 19, 7, 8, 9, 20]  # :254
@@ -26,17 +31,23 @@ TIPS = {"right": [745, 317, 444, 556, 673], "left": [745, 317, 445, 556, 673]}  
 
 
 def _with_zeros(m34):
-    pad = np.zeros((m34.shape[0], 1, 4), F)
+    pad = np.zeros((m34.shape[0], 1, 4), m34.dtype)
     pad[:, 0, 3] = 1
     return np.concatenate([m34, pad], 1)
 
 
-def mano_forward(asset, pose, betas, side, center_idx=9, flip_shapedirs_x=None):
+def mano_forward(asset, pose, betas, side, center_idx=9, flip_shapedirs_x=None, dtype=None, detail=None):
     """pose (n,48) axis-angle [root3 | hand45], betas (n,10) -> verts (n,778,3),
     joints (n,21,3), center (n,1,3).
 
     ``flip_shapedirs_x`` defaults to ``side == 'left'`` which is what MANOWrapper does
-    to the left layer after construction (acr/mano_wrapper.py:35)."""
+    to the left layer after construction (acr/mano_wrapper.py:35).
+    ``dtype`` is the type of every operation: float32 (the default, which the goldens pin) is the reference's;
+    float64 is the statement the kernels' per-element bounds are taken against (tests/tail_ref.py).  A dict passed
+    as ``detail`` receives the intermediates those bounds are built from: full_pose (n,16,3), R (n,16,3,3) local
+    rotations, J (n,16,3) rest joints, v_posed (n,778,3), G (n,16,4,4) global transforms, A (n,16,4,4) with the rest
+    pose removed, and the model arrays as used (shapedirs after the flip)."""
+    F = _dtype(dtype)
     pose = np.asarray(pose, F).reshape(-1, 48)
     betas = np.asarray(betas, F).reshape(-1, 10)
     n = pose.shape[0]
@@ -54,7 +65,7 @@ def mano_forward(asset, pose, betas, side, center_idx=9, flip_shapedirs_x=None):
     # (i) full pose = [root | mean + hand]            manolayer.py:125-137
     full = np.concatenate([pose[:, :3], hands_mean[None] + pose[:, 3:]], 1).astype(F)
     # (ii) 16 rotations; pose_map = R - I for joints 1..15      :140-143, 281-287
-    rots = batch_rodrigues(full.reshape(-1, 3)).reshape(n, 16, 9)
+    rots = batch_rodrigues(full.reshape(-1, 3), F).reshape(n, 16, 9)
     root_rot = rots[:, 0].reshape(n, 3, 3)
     rot_map = rots[:, 1:].reshape(n, 135)
     pose_map = rot_map - np.tile(np.eye(3, dtype=F).reshape(9), 15)[None]
@@ -90,6 +101,9 @@ def mano_forward(asset, pose, betas, side, center_idx=9, flip_shapedirs_x=None):
     jtr = np.concatenate([G[:, :, :3, 3], verts[:, TIPS[side]]], 1)
     # (xi) reorder, (xii) centre on joint ``center_idx``         :254-261
     jtr = jtr[:, JOINT_REORDER]
+    if detail is not None:
+        detail.update(full_pose=full.reshape(n, 16, 3), R=rots.reshape(n, 16, 3, 3), J=J, v_posed=v_posed, G=G, A=G2,
+                      shapedirs=shapedirs, posedirs=posedirs, v_template=v_template, J_regressor=Jreg, weights=weights)
     center = None
     if center_idx is not None:
         center = jtr[:, center_idx][:, None].copy()

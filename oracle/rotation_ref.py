@@ -18,15 +18,23 @@ import numpy as np
 F = np.float32
 
 
+def _dtype(dtype):
+    """The type a function computes in: its ``dtype`` argument, or the module's F (float32, the reference's)."""
+    return globals()["F"] if dtype is None else dtype
+
+
 def _normalize(v, eps):
     # torch.nn.functional.normalize: v / max(||v||, eps)
+    F = v.dtype.type
     n = np.sqrt((v * v).sum(-1, keepdims=True, dtype=F))
     return v / np.maximum(n, F(eps))
 
 
-def rot6d_to_rotmat(x):
+def rot6d_to_rotmat(x, dtype=None):
     """(M,6) -> (M,3,3); the 6 numbers are read as a row-major (3,2) matrix whose two
-    columns are the raw basis vectors (acr/utils.py:363 ``x.view(-1,3,2)``)."""
+    columns are the raw basis vectors (acr/utils.py:363 ``x.view(-1,3,2)``).
+    ``dtype`` (here and below): the type of every operation, float32 like the reference or float64."""
+    F = _dtype(dtype)
     x = np.asarray(x, F).reshape(-1, 3, 2)
     a1, a2 = x[:, :, 0], x[:, :, 1]
     b1 = _normalize(a1, 1e-6)
@@ -36,9 +44,10 @@ def rot6d_to_rotmat(x):
     return np.stack([b1, b2, b3], axis=-1)  # columns b1,b2,b3
 
 
-def rotmat_to_quaternion(R, eps=1e-6):
+def rotmat_to_quaternion(R, eps=1e-6, dtype=None):
     """(M,3,3) -> (M,4) wxyz; 4-case selection evaluated on the TRANSPOSED matrix
     (acr/utils.py:862 ``rmat_t = transpose(rotation_matrix)``)."""
+    F = _dtype(dtype)
     R = np.asarray(R, F)
     t = np.transpose(R, (0, 2, 1))
     m = lambda i, j: t[:, i, j]
@@ -64,7 +73,8 @@ def rotmat_to_quaternion(R, eps=1e-6):
     return q.astype(F)
 
 
-def quaternion_to_angle_axis(q):
+def quaternion_to_angle_axis(q, dtype=None):
+    F = _dtype(dtype)
     q = np.asarray(q, F)
     q1, q2, q3 = q[:, 1], q[:, 2], q[:, 3]
     s2 = q1 * q1 + q2 * q2 + q3 * q3
@@ -76,8 +86,8 @@ def quaternion_to_angle_axis(q):
     return np.stack([q1 * k, q2 * k, q3 * k], -1).astype(F)
 
 
-def rotmat_to_angle_axis(R):
-    aa = quaternion_to_angle_axis(rotmat_to_quaternion(R))
+def rotmat_to_angle_axis(R, dtype=None):
+    aa = quaternion_to_angle_axis(rotmat_to_quaternion(R, dtype=dtype), dtype)
     aa[np.isnan(aa)] = 0.0
     return aa
 
@@ -89,9 +99,11 @@ def rot6d_to_angular(rot6d):
     return rotmat_to_angle_axis(rot6d_to_rotmat(rot6d.reshape(-1, 6))).reshape(n, -1)
 
 
-def batch_rodrigues(aa):
+def batch_rodrigues(aa, dtype=None):
     """(M,3) -> (M,9) row-major rotation, via the half-angle quaternion with the
-    reference's 1e-8 offset inside the norm (mano/manolayer.py:425)."""
+    reference's 1e-8 offset inside the norm (mano/manolayer.py:425).  ``dtype`` is the type of every
+    operation: float32 is the reference's, float64 the high-precision statement the kernels are bounded against."""
+    F = _dtype(dtype)
     aa = np.asarray(aa, F)
     ang = np.sqrt(((aa + F(1e-8)) ** 2).sum(-1, keepdims=True, dtype=F))
     axis = aa / ang
