@@ -39,6 +39,9 @@ _DEFAULTS = dict(
     mano_mesh_root_align=True,                             # configs/demo.yml:11
     val_batch_size=1, GPUS="0",                            # configs/demo.yml:3,8
     temporal_optimization=False, smooth_coeff=4.0,         # config.py:29-30
+    track_hands=False, track_gate=8, track_max_missed=15,  # multi-hand tracking in process_results (DESIGN.md): track ids,
+                                                          # and with temporal_optimization one filter bank per track;
+                                                          # gate in centre-map cells, max_missed in frames
     model_path=os.path.join(project_dir, "checkpoints", "wild.pkl"),
     mano_root=os.path.join(project_dir, "mano"),           # acr/mano_wrapper.py:22 uses 'mano/'
     cam_trans_mode="lstsq",                                # 'lstsq' (device least squares, SURVEY 8f-1) | 'pnp' (device

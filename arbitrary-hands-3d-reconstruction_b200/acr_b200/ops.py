@@ -241,6 +241,71 @@ def one_euro_smooth(poses: torch.Tensor, betas: torch.Tensor, state: OneEuroStat
                                                       L.current_stream(dev)), "one_euro_smooth")
 
 
+class HandTracker:
+    """Device-side state of multi-hand tracking for one stream (acr_b200_track_hands): K track slots per side, each
+    with its id, last cell, missed-frame count and OneEuro bank.  ``gate`` is in centre-map cells (8 cells = 64 px
+    on the 512 input; >= 90 never rejects), ``max_missed`` in frames (15 = half a second at 30 fps);
+    ``smooth_coeff`` None tracks ids only, a positive value also filters poses and betas per track.  Owns one (2KB,)
+    int32 id buffer per batch size, reused by every call (zero copy, like ParseBuffers)."""
+
+    def __init__(self, device, K: int, gate: int = 8, max_missed: int = 15, smooth_coeff: Optional[float] = 4.0):
+        if not 1 <= int(K) <= MAX_HANDS_PER_SIDE:
+            raise ValueError(f"hands per side must be in 1..{MAX_HANDS_PER_SIDE}, got {K}")
+        if int(gate) < 0 or int(max_missed) < 0:
+            raise ValueError(f"gate and max_missed must be >= 0, got {gate}, {max_missed}")
+        if smooth_coeff is not None and not float(smooth_coeff) > 0:
+            raise ValueError(f"smooth_coeff must be positive or None, got {smooth_coeff}")
+        self.device, self.K, self.gate, self.max_missed = torch.device(device), int(K), int(gate), int(max_missed)
+        self.smooth_coeff = None if smooth_coeff is None else float(smooth_coeff)
+        self.state = torch.zeros(int(L.load().acr_b200_track_state_bytes(self.K)), dtype=torch.uint8,
+                                 device=self.device)
+        self._ids = {}
+
+    def ids(self, B: int) -> torch.Tensor:
+        """The (2KB,) id buffer of batch size B."""
+        if B not in self._ids:
+            self._ids[B] = torch.full((2 * self.K * B,), -1, dtype=torch.int32, device=self.device)
+        return self._ids[B]
+
+    def reset(self) -> None:
+        """No tracks, birth counters at zero; in place, so a captured graph stays valid."""
+        self.state.zero_()
+
+
+def track_rows(tracker: HandTracker, B: int, row_src: torch.Tensor, detection_flag: Optional[torch.Tensor],
+               poses: Optional[torch.Tensor] = None, betas: Optional[torch.Tensor] = None,
+               n_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Track the rows of B consecutive frames (``row_src`` (n,4) int32 in the parse's layout, n <= 2KB) on the current
+    stream, no host sync.  With the tracker's ``smooth_coeff`` set, ``poses`` (n,48) and ``betas`` (n,10) (contiguous
+    fp32) are filtered in place.  Returns the tracker's id buffer for B; rows [0, min(n, n_dev)) are valid."""
+    dev = L.require_cuda(row_src, detection_flag, poses, betas, n_dev, tracker.state)
+    n = row_src.shape[0]
+    assert row_src.dtype == torch.int32 and row_src.is_contiguous() and row_src.shape[1:] == (4,)
+    assert detection_flag is None or (detection_flag.dtype == torch.float32 and detection_flag.is_contiguous())
+    smooth = tracker.smooth_coeff is not None
+    if smooth:
+        assert poses is not None and betas is not None, "a smoothing tracker needs poses and betas"
+        assert poses.is_contiguous() and betas.is_contiguous() and poses.dtype == betas.dtype == torch.float32
+    ids = tracker.ids(B)
+    with L.on(dev):
+        L.check(L.load().acr_b200_track_hands(L.ptr(poses) if smooth else None, L.ptr(betas) if smooth else None,
+                                              L.ptr(row_src), L.ptr(detection_flag), L.ptr(n_dev), n, int(B),
+                                              tracker.K, tracker.gate, tracker.max_missed,
+                                              tracker.smooth_coeff or 0.0, L.ptr(tracker.state), L.ptr(ids),
+                                              L.current_stream(dev)), "track_hands")
+    return ids
+
+
+def track_hands(bufs: "ParseBuffers", tracker: HandTracker) -> torch.Tensor:
+    """Track the hands of a parse (ParseBuffers of B consecutive frames of one stream) on the current stream, no host
+    sync: poses / betas are filtered in place when the tracker smooths (params_pred, global_orient and hand_pose stay
+    raw).  Returns the tracker's (2KB,) int32 id buffer, valid over rows [0, counts[2])."""
+    if tracker.K != bufs.K:
+        raise ValueError(f"this tracker is built for K={tracker.K}, the parse buffers for K={bufs.K}")
+    return track_rows(tracker, bufs.B, bufs.row_src, bufs.detection_flag, bufs.poses, bufs.betas,
+                      n_dev=bufs.counts[2:3])
+
+
 # ------------------------------------------------------------------------------ rotations
 def rot6d_to_aa(rot6d: torch.Tensor) -> torch.Tensor:
     """(N, 6*J) -> (N, 3*J); drop-in for acr.utils.rot6D_to_angular."""

@@ -9,18 +9,13 @@
 //   alpha(c) = 1 / (1 + (1/(2 pi c)) / (1/freq)),  freq = 30, beta = 0.7, dcutoff = 1,
 //   mincutoff = smooth_coeff (pose, root rotation) | 0.6 (betas).
 #include "common.cuh"
+#include "one_euro.cuh"
 #include "rotation.cuh"
 
 namespace acr {
 
 constexpr int SM_ELEMS = 64;            // 45 pose + 10 betas + 9 rotation entries
 constexpr int SM_STATE = 4 * SM_ELEMS;  // per hand type: prev_raw, prev_filtered, prev_filtered_dx, [0] = initialised
-
-__device__ __forceinline__ float one_euro_alpha(float cutoff) {
-  const float te = 1.0f / 30.0f;
-  const float tau = 1.0f / (2.0f * 3.14159265358979323846f * cutoff);
-  return 1.0f / (1.0f + tau / te);
-}
 
 __global__ void __launch_bounds__(SM_ELEMS) one_euro_kernel(float* __restrict__ poses, float* __restrict__ betas,
                                                             const int32_t* __restrict__ hand_type,
@@ -42,13 +37,7 @@ __global__ void __launch_bounds__(SM_ELEMS) one_euro_kernel(float* __restrict__ 
   const bool init = st[3 * SM_ELEMS] != 0.f;
   float xh, edx;
   if (!init) { xh = x; edx = 0.f; }
-  else {
-    const float dx = (x - st[e]) * 30.0f;
-    const float ad = one_euro_alpha(1.0f);
-    edx = ad * dx + (1.0f - ad) * st[2 * SM_ELEMS + e];
-    const float a = one_euro_alpha(mincut + 0.7f * fabsf(edx));
-    xh = a * x + (1.0f - a) * st[SM_ELEMS + e];
-  }
+  else one_euro_step(x, mincut, st[e], st[SM_ELEMS + e], st[2 * SM_ELEMS + e], xh, edx);
   __syncthreads();   // every thread has read the init flag and its old state
   st[e] = x; st[SM_ELEMS + e] = xh; st[2 * SM_ELEMS + e] = edx;
   if (e == 0) st[3 * SM_ELEMS] = 1.f;

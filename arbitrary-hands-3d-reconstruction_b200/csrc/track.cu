@@ -1,0 +1,328 @@
+// Multi-hand tracking between parse and MANO: a stable track id per detected hand and one OneEuro bank per track,
+// for up to K hands per side, over B consecutive frames of one stream in one launch.  The statement (matching,
+// misses, births, ids, filtering) is tests/track_ref.py; DESIGN.md "Multi-hand tracking" gives the reasons.
+//
+// One CTA per side; the state is per side: a header (birth counter), K slot records (id, cell, missed, live) and K
+// banks of 3 x 64 floats (previous raw value, filtered value, filtered derivative of the 45 pose values, 10 betas
+// and 9 root-matrix entries, acr_b200_one_euro_smooth's layout).  Frames go in chunks of TR_CHUNK:
+//   association  warp 0 walks the row table in windows of 32 rows (coalesced), keeps a side's rows whose images
+//                do not go back in time, and runs match / miss / birth per frame with the K slots in lanes 0..K-1
+//                and the frame's detections in lanes 0..nd-1; the match takes the smallest packed key
+//                (d2 << 8 | slot << 4 | rank) per round, a total order, with one warp min-reduction.  It writes each
+//                row's id and, per frame of the chunk, the row of every slot and the births.
+//   filter       thread (slot k, element e) keeps bank element e of slot k in registers and walks the chunk's
+//                frames in order: the only serial recurrence.  The chunk's inputs are loaded first, all at once.
+//   root         one thread per (frame, slot) turns the filtered root matrix back into an axis angle; it overlaps
+//                the association of the next chunk (warp 0).
+// No atomics; every result is written by one thread in a fixed order, so repeated launches are bit-identical and
+// one launch over B frames equals B launches of one frame.
+#include "common.cuh"
+#include "one_euro.cuh"
+#include "rotation.cuh"
+
+namespace acr {
+
+constexpr int TR_MAX_K = 16;
+constexpr int TR_ELEMS = 64;          // 45 pose + 10 betas + 9 root-matrix entries
+constexpr int TR_CHUNK = 8;           // frames per association / filter phase (16 spills at 64 registers)
+constexpr int TR_NCELL = 64 * 64;     // flat cells of the centre map
+constexpr unsigned FULL = 0xffffffffu;
+
+struct TrackSlot {
+  int32_t id, cell, missed, live;
+};
+
+// per side: int32 births, 3 pad, TrackSlot[K], float bank[K][3][64]
+__host__ __device__ constexpr size_t track_side_bytes(int K) {
+  return 16 + (size_t)K * sizeof(TrackSlot) + (size_t)K * 3 * TR_ELEMS * sizeof(float);
+}
+
+template <bool kPiTrig>
+__device__ __forceinline__ float rodrigues_entry(float ax, float ay, float az, int j) {
+  float R[9];
+  rodrigues<kPiTrig>(ax, ay, az, R);
+  float x = R[0];
+#pragma unroll
+  for (int i = 1; i < 9; ++i)
+    if (j == i) x = R[i];
+  return x;
+}
+
+// Entry j of rodrigues() as acr_b200_one_euro_smooth evaluates it (sincosf).  sincosf's reduction for |angle / 2|
+// >= 105615 keeps a scratch array in local memory; such angles (beyond 2e5 rad) take the sincospif form instead,
+// which needs none.  The test is sincosf's own, so the compiler drops that reduction from the first branch.
+__device__ __forceinline__ float track_rodrigues_entry(float ax, float ay, float az, int j) {
+  const float bx = ax + 1e-8f, by = ay + 1e-8f, bz = az + 1e-8f;
+  const float half = sqrtf(bx * bx + by * by + bz * bz) * 0.5f;
+  return !(fabsf(half) >= 105615.0f) ? rodrigues_entry<false>(ax, ay, az, j) : rodrigues_entry<true>(ax, ay, az, j);
+}
+
+struct TrackParams {
+  float* poses;
+  float* betas;
+  const int32_t* row_src;
+  const float* flag;
+  const int32_t* n_dev;
+  int n_max, B, K, gate2, max_missed;
+  float smooth_coeff;
+  char* state;
+  int32_t* track_id;
+};
+
+__global__ void __launch_bounds__(TR_MAX_K * TR_ELEMS) track_kernel(TrackParams q) {
+  __shared__ int s_row[2][TR_CHUNK][TR_MAX_K];     // row of slot k in frame f of the chunk, -1: none
+  __shared__ unsigned s_born[2][TR_CHUNK];         // bit k: slot k's track is born in frame f
+  __shared__ float s_R[TR_CHUNK][TR_MAX_K][9];     // filtered root matrices of the chunk
+  const int side = blockIdx.x, t = threadIdx.x, lane = t & 31, K = q.K, B = q.B;
+  const bool smooth = q.poses != nullptr;
+  const int n = max(0, q.n_dev ? min(*q.n_dev, q.n_max) : q.n_max);
+  char* st = q.state + (size_t)side * track_side_bytes(K);
+  int32_t* hdr = reinterpret_cast<int32_t*>(st);
+  TrackSlot* slots = reinterpret_cast<TrackSlot*>(st + 16);
+  float* banks = reinterpret_cast<float*>(st + 16 + (size_t)K * sizeof(TrackSlot));
+
+  // rows of no side and rows at or past n: id -1 (the side CTAs write every other row)
+  if (side == 0)
+    for (int r = t; r < q.n_max; r += blockDim.x)
+      if (r >= n || (unsigned)q.row_src[(size_t)r * 4 + 1] > 1u) q.track_id[r] = -1;
+
+  // ---- filter thread: bank element e of slot k
+  const int k = t >> 6, e = t & 63;
+  float raw = 0.f, filt = 0.f, fdx = 0.f;
+  const float mincut = (e >= 45 && e < 55) ? 0.6f : q.smooth_coeff;
+  if (smooth) {
+    const float* bk = banks + (size_t)k * 3 * TR_ELEMS;
+    raw = bk[e]; filt = bk[TR_ELEMS + e]; fdx = bk[2 * TR_ELEMS + e];
+  }
+
+  // ---- association warp: slot k in lane k, the row window in lanes
+  int s_live = 0, s_id = 0, s_cell = 0, s_missed = 0, births = 0;
+  int win_base = -32, w_img = 0, w_cell = 0, runmax = -1;
+  bool w_det = false;
+  if (t < 32) {
+    births = hdr[0];
+    if (lane < K) {
+      const TrackSlot sl = slots[lane];
+      s_id = sl.id; s_cell = sl.cell; s_missed = sl.missed; s_live = sl.live != 0;
+    }
+  }
+
+  // load rows [win_base, win_base + 32): a row of this side is kept when its image is in [0, B), its cell on the map
+  // and its image not below any earlier kept row's (the prefix max of in-range images; an out-of-order row cannot
+  // raise it); a kept row with detection_flag > 0 is a detection, every other row of this side gets id -1 here
+  auto load_window = [&]() {
+    const int r = win_base + lane;
+    int rs = -1, img = 0, cell = 0;
+    float fl = 1.f;
+    if (r < n) {
+      const int32_t* p = q.row_src + (size_t)r * 4;
+      img = p[0]; rs = p[1]; cell = p[2];
+      if (q.flag) fl = q.flag[r];
+    }
+    const bool inr = rs == side && img >= 0 && img < B && cell >= 0 && cell < TR_NCELL;
+    int v = inr ? img : -1;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const int o = __shfl_up_sync(FULL, v, off);
+      if (lane >= off) v = max(v, o);
+    }
+    int before = __shfl_up_sync(FULL, v, 1);
+    if (lane == 0) before = -1;
+    const bool kept = inr && img >= max(runmax, before);
+    runmax = max(runmax, __shfl_sync(FULL, v, 31));
+    w_det = kept && fl > 0.f;
+    w_img = img; w_cell = cell;
+    if (rs == side && !w_det) q.track_id[r] = -1;
+  };
+
+  auto associate_frame = [&](int f, int fi, int buf) {
+    // 1. the frame's detections, in row order, into lanes 0..nd-1 (beyond K: id -1)
+    int nd = 0, d_row = -1, d_cell = 0;
+    while (true) {
+      const unsigned m = __ballot_sync(FULL, w_det);
+      if (m == 0) {
+        if (win_base + 32 >= n) break;
+        win_base += 32;
+        load_window();
+        continue;
+      }
+      const int j = __ffs(m) - 1;
+      if (__shfl_sync(FULL, w_img, j) != f) break;       // a later frame's
+      const int cj = __shfl_sync(FULL, w_cell, j), rj = win_base + j;
+      if (lane == j) w_det = false;
+      if (nd < K) {
+        if (lane == nd) { d_row = rj; d_cell = cj; }
+        ++nd;
+      } else if (lane == 0) {
+        q.track_id[rj] = -1;
+      }
+    }
+    // 2. match: pairs (slot, detection) within the gate, smallest (d2, slot, rank) first
+    unsigned key[TR_MAX_K * TR_MAX_K / 32];
+#pragma unroll
+    for (int i = 0; i < TR_MAX_K * TR_MAX_K / 32; ++i) {
+      const int p = lane + 32 * i, kk = p >> 4, d = p & 15;
+      const int sc = __shfl_sync(FULL, s_cell, kk), sl = __shfl_sync(FULL, s_live, kk);
+      const int dc = __shfl_sync(FULL, d_cell, d);
+      const int dy = (sc >> 6) - (dc >> 6), dx = (sc & 63) - (dc & 63), d2 = dy * dy + dx * dx;
+      key[i] = (kk < K && d < nd && sl && d2 <= q.gate2) ? ((unsigned)d2 << 8 | (unsigned)kk << 4 | (unsigned)d) : ~0u;
+    }
+    unsigned mslot = 0, mdet = 0;
+    int k_det = -1, d_slot = -1;        // lane k: the detection slot k takes; lane d: the slot detection d goes to
+    while (true) {
+      unsigned best = ~0u;
+#pragma unroll
+      for (int i = 0; i < TR_MAX_K * TR_MAX_K / 32; ++i) {
+        const unsigned kk = (key[i] >> 4) & 15u, d = key[i] & 15u;
+        if (key[i] < best && !((mslot >> kk) & 1u) && !((mdet >> d) & 1u)) best = key[i];
+      }
+      best = __reduce_min_sync(FULL, best);
+      if (best == ~0u) break;
+      const int kk = (best >> 4) & 15, d = best & 15;
+      mslot |= 1u << kk; mdet |= 1u << d;
+      if (lane == kk) k_det = d;
+      if (lane == d) d_slot = kk;
+    }
+    // 3. misses: a matched slot follows its detection, an unmatched one is freed past max_missed
+    const int mcell = __shfl_sync(FULL, d_cell, k_det & 31);
+    if (lane < K && s_live) {
+      if ((mslot >> lane) & 1u) { s_missed = 0; s_cell = mcell; }
+      else if (s_missed >= q.max_missed) s_live = 0;
+      else ++s_missed;
+    }
+    // 4. births in row order: the lowest free slot, else the most-missed slot not matched or born in this frame
+    unsigned todo = ~mdet & ((1u << nd) - 1u), bornm = 0;
+    while (todo) {
+      const int d = __ffs(todo) - 1;
+      todo &= todo - 1;
+      const int dc = __shfl_sync(FULL, d_cell, d);
+      const unsigned freem = __ballot_sync(FULL, lane < K && !s_live);
+      int kk;
+      if (freem) {
+        kk = __ffs(freem) - 1;
+      } else {
+        const bool cand = lane < K && !(((mslot | bornm) >> lane) & 1u);
+        const int most = __reduce_max_sync(FULL, cand ? s_missed : -1);
+        kk = __ffs(__ballot_sync(FULL, cand && s_missed == most)) - 1;
+      }
+      if (lane == kk) { s_live = 1; s_id = 2 * births + side; s_cell = dc; s_missed = 0; k_det = d; }
+      if (lane == d) d_slot = kk;
+      ++births;
+      bornm |= 1u << kk;
+    }
+    // 5. outputs: the ids, and the frame's row per slot for the filter
+    const int rowk = __shfl_sync(FULL, d_row, k_det & 31);
+    if (lane < TR_MAX_K) s_row[buf][fi][lane] = (lane < K && k_det >= 0) ? rowk : -1;
+    if (lane == 0) s_born[buf][fi] = bornm;
+    const int idd = __shfl_sync(FULL, s_id, d_slot & 31);
+    if (lane < nd) q.track_id[d_row] = idd;
+  };
+
+  auto associate_chunk = [&](int c) {
+    const int buf = c & 1;
+    for (int fi = 0; fi < TR_CHUNK; ++fi) {
+      const int f = c * TR_CHUNK + fi;
+      if (f < B) associate_frame(f, fi, buf);
+      else if (lane < TR_MAX_K) s_row[buf][fi][lane] = -1;
+    }
+  };
+
+  // step c: filter chunk c - 1, then associate chunk c while the root pass finishes chunk c - 1
+  const int nch = (B + TR_CHUNK - 1) / TR_CHUNK;
+  for (int c = 0; c <= nch; ++c) {
+    const int buf = (c - 1) & 1;
+    if (smooth && c > 0) {
+      // the chunk's inputs first (independent loads), then the recurrence; lanes e = 55..57 hold the root's axis
+      // angle, from which every root-matrix lane of the warp computes the Rodrigues matrix
+      float xs[TR_CHUNK];
+#pragma unroll
+      for (int fi = 0; fi < TR_CHUNK; ++fi) {
+        const int r = s_row[buf][fi][k];
+        xs[fi] = 0.f;
+        if (r >= 0) {
+          if (e < 45) xs[fi] = q.poses[(size_t)r * 48 + 3 + e];
+          else if (e < 55) xs[fi] = q.betas[(size_t)r * 10 + (e - 45)];
+          else if (e < 58) xs[fi] = q.poses[(size_t)r * 48 + (e - 55)];
+        }
+      }
+#pragma unroll
+      for (int fi = 0; fi < TR_CHUNK; ++fi) {
+        const int r = s_row[buf][fi][k];                 // uniform over the slot's two warps
+        if (r < 0) continue;
+        float x = xs[fi];
+        if (e >= 32) {
+          const float ax = __shfl_sync(FULL, x, 23), ay = __shfl_sync(FULL, x, 24), az = __shfl_sync(FULL, x, 25);
+          if (e >= 55) x = track_rodrigues_entry(ax, ay, az, e - 55);
+        }
+        float xh = x, edx = 0.f;                          // a newborn track's first frame passes through
+        const bool born = (s_born[buf][fi] >> k) & 1u;
+        if (!born) one_euro_step(x, mincut, raw, filt, fdx, xh, edx);
+        raw = x; filt = xh; fdx = edx;
+        if (e >= 55) s_R[fi][k][e - 55] = xh;
+        else if (!born) {
+          if (e < 45) q.poses[(size_t)r * 48 + 3 + e] = xh;
+          else q.betas[(size_t)r * 10 + (e - 45)] = xh;
+        }
+      }
+    }
+    __syncthreads();
+    if (t < 32) {
+      if (c < nch) associate_chunk(c);
+    } else if (smooth && c > 0 && t - 32 < TR_CHUNK * K) {
+      const int fi = (t - 32) / K, kk = (t - 32) % K;
+      const int r = s_row[buf][fi][kk];
+      if (r >= 0) {
+        float aa[3];
+        rotmat_to_aa(&s_R[fi][kk][0], aa);
+        q.poses[(size_t)r * 48 + 0] = aa[0]; q.poses[(size_t)r * 48 + 1] = aa[1]; q.poses[(size_t)r * 48 + 2] = aa[2];
+      }
+    }
+    __syncthreads();
+  }
+
+  if (smooth) {
+    float* bk = banks + (size_t)k * 3 * TR_ELEMS;
+    bk[e] = raw; bk[TR_ELEMS + e] = filt; bk[2 * TR_ELEMS + e] = fdx;
+  }
+  if (t < 32) {
+    if (lane == 0) hdr[0] = births;
+    if (lane < K) {
+      TrackSlot sl;
+      sl.id = s_id; sl.cell = s_cell; sl.missed = s_missed; sl.live = s_live;
+      slots[lane] = sl;
+    }
+  }
+}
+
+}  // namespace acr
+
+using namespace acr;
+
+extern "C" size_t acr_b200_track_state_bytes(int K) {
+  return (K >= 1 && K <= TR_MAX_K) ? 2 * track_side_bytes(K) : 0;
+}
+
+extern "C" int acr_b200_track_hands(float* poses, float* betas, const int32_t* row_src, const float* detection_flag,
+                                    const int32_t* n_dev, int n_max, int B, int K, int gate, int max_missed,
+                                    float smooth_coeff, void* state, int32_t* track_id, void* stream) {
+  ACR_CHECK_ARG(K >= 1 && K <= TR_MAX_K, "track_hands: K must be in 1..%d (got %d)", TR_MAX_K, K);
+  ACR_CHECK_ARG(B >= 1, "track_hands: B must be positive (got %d)", B);
+  ACR_CHECK_ARG(n_max >= 0 && (long long)n_max <= 2LL * K * B, "track_hands: n_max must be in 0..2*K*B = %lld (got %d)",
+                2LL * K * B, n_max);
+  ACR_CHECK_ARG(gate >= 0 && max_missed >= 0, "track_hands: gate and max_missed must be >= 0 (got %d, %d)", gate,
+                max_missed);
+  ACR_CHECK_ARG(state && row_src && track_id, "track_hands: null state, row table or id buffer");
+  ACR_CHECK_ARG((poses == nullptr) == (betas == nullptr), "track_hands: poses and betas must be both given or both NULL");
+  const bool smooth = poses != nullptr;
+  ACR_CHECK_ARG(!smooth || smooth_coeff > 0.f, "track_hands: smooth_coeff must be positive when smoothing");
+  TrackParams q;
+  q.poses = poses; q.betas = betas; q.row_src = row_src; q.flag = detection_flag; q.n_dev = n_dev;
+  q.n_max = n_max; q.B = B; q.K = K;
+  q.gate2 = min(gate, 90) * min(gate, 90);     // 63^2 + 63^2 < 90^2: a wider gate rejects nothing more
+  q.max_missed = max_missed; q.smooth_coeff = smooth_coeff;
+  q.state = static_cast<char*>(state); q.track_id = track_id;
+  // ids only: the association warp alone
+  track_kernel<<<2, smooth ? K * TR_ELEMS : 32, 0, (cudaStream_t)stream>>>(q);
+  ACR_CHECK_LAUNCH();
+  return ACR_B200_OK;
+}

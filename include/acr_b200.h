@@ -239,6 +239,26 @@ size_t acr_b200_one_euro_state_floats(void);
 int acr_b200_one_euro_smooth(float* poses, float* betas, const int32_t* hand_type, const float* detection_flag,
                              const int32_t* n_dev, int n_max, float* state, float smooth_coeff, void* stream);
 
+/* Multi-hand tracking of one stream between parse and MANO: a stable track id per detected hand and one OneEuro
+ * bank per track, for up to K hands per side (the parse's max_hands_per_side).  The B images of a call are B
+ * consecutive frames in time order; rows are in the parse's layout (row_src (n,4): image, side, flat centre cell
+ * y*64+x, unused).  Per frame and side: live tracks match detections greedily by integer squared cell distance
+ * within `gate` cells (ties by slot, then row); a track unmatched for more than `max_missed` consecutive frames
+ * ends; an unmatched detection starts a track in the lowest free slot, or replaces the most-missed unmatched one.
+ * Track ids are 2*c + side with a per-side birth counter c, never reused.  tests/track_ref.py is the statement.
+ * track_id (n_max) gets each row's id, -1 for a row that is no detection (detection_flag <= 0, at or past *n_dev,
+ * out of range, or out of time order -- such rows are left untouched).  With poses (n,48) and betas (n,10), each
+ * tracked detection is filtered in place through its track's bank with acr_b200_one_euro_smooth's arithmetic (a
+ * track's first frame passes the pose's 45 values and the betas through); with both NULL only ids are computed.
+ * `state`: device buffer of acr_b200_track_state_bytes(K) bytes, zeroed = no tracks.  One launch over B frames
+ * equals B launches of one frame, bit for bit.  K outside 1..16, B < 1, n_max outside 0..2*K*B, gate or max_missed
+ * < 0, a NULL state / row_src / track_id, exactly one of poses and betas NULL, or smooth_coeff <= 0 with poses is
+ * ACR_B200_EINVAL and nothing is launched.  acr_b200_track_state_bytes returns 0 for K outside 1..16.          */
+size_t acr_b200_track_state_bytes(int K);
+int acr_b200_track_hands(float* poses, float* betas, const int32_t* row_src, const float* detection_flag,
+                         const int32_t* n_dev, int n_max, int B, int K, int gate, int max_missed, float smooth_coeff,
+                         void* state, int32_t* track_id, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Rotations
  * ---------------------------------------------------------------------------------------- */
