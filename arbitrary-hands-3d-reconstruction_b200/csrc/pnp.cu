@@ -17,7 +17,9 @@
 // The SVDs are one-sided Jacobi with OpenCV's rotation rule and threshold, and, as in OpenCV, the singular vectors
 // EPnP uses are the normalised rotated columns.  The hypothesis' rotation is used as a matrix (OpenCV's Rodrigues
 // round trip moves it by an ulp).  Exactly 4 usable joints would be OpenCV's P3P; this path returns the least
-// squares there instead.
+// squares there instead.  Planar or collinear usable joints have no EPnP control points: such a hypothesis has no
+// inliers, and a final or 5-point fit on them returns the least squares with mask 0 (OpenCV carries on with a
+// pseudo-inverse, in a null space where round-off decides the answer).
 #include <float.h>
 
 #include "common.cuh"
@@ -362,7 +364,8 @@ __device__ __forceinline__ double r_and_t(const PnpSmem& sm, bool has, int np, c
 }
 
 // EPnP on np <= 21 points, this lane's point (X, Y, Z) -> pixel (u, v) if lane < np; K = [f 0 c; 0 f c; 0 0 1].
-// The pose goes to sm.R, sm.t.
+// The pose goes to sm.R, sm.t; t is NaN when the points are planar or collinear (the smallest eigenvalue of their
+// covariance at most 10 eps of the largest), where the control-point matrix has no inverse.
 __device__ void epnp(PnpSmem& sm, int lane, int np, double X, double Y, double Z, double u, double v, double f,
                      double c) {
   __syncwarp();
@@ -377,6 +380,11 @@ __device__ void epnp(PnpSmem& sm, int lane, int np, double X, double Y, double Z
 #pragma unroll
     for (int j = i; j < 3; ++j) At[i][j] = At[j][i] = wsum(d[i] * d[j]);
   svd3(At, dc, Vt);
+  if (!(dc[2] > JAC_EPS * dc[0])) {   // planar or collinear points: no control points, no alphas (warp-uniform)
+    if (lane == 0) sm.t[0] = sm.t[1] = sm.t[2] = __longlong_as_double(0x7ff8000000000000ll);
+    __syncwarp();
+    return;
+  }
   double cws[4][3];
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -514,6 +522,19 @@ __device__ __forceinline__ bool is_inlier(const double (&R)[3][3], const double 
   return __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) <= THRESH2;
 }
 
+// the EPnP answer and its inlier mask; a non-finite t (EPnP failed) takes the least squares and mask 0, as when
+// RANSAC finds no consensus
+__device__ __forceinline__ void store_epnp(const PnpSmem& sm, const float* jh, const float* ph, float focal,
+                                           float img_size, float* o, int32_t* inl, unsigned joints) {
+  if (isfinite(sm.t[0]) && isfinite(sm.t[1]) && isfinite(sm.t[2])) {
+    o[0] = (float)sm.t[0]; o[1] = (float)sm.t[1]; o[2] = (float)sm.t[2];
+  } else {
+    cam_trans_lstsq(jh, ph, focal, img_size, o);
+    joints = 0;
+  }
+  if (inl) *inl = (int32_t)joints;
+}
+
 __global__ void __launch_bounds__(PNP_WARPS * 32)
 cam_trans_pnp_kernel(const float* __restrict__ j3d, const float* __restrict__ pj2d, const int32_t* __restrict__ n_dev,
                      int n_max, float focal, float img_size, float* __restrict__ out, int32_t* __restrict__ inl_out) {
@@ -557,10 +578,7 @@ cam_trans_pnp_kernel(const float* __restrict__ j3d, const float* __restrict__ pj
     epnp(sm, lane, cnt, has ? sm.S[lane][0] : 0.f, has ? sm.S[lane][1] : 0.f, has ? sm.S[lane][2] : 0.f,
          has ? pix_fp32_normalised(sm.J[lane][0], f, c) : 0.0, has ? pix_fp32_normalised(sm.J[lane][1], f, c) : 0.0,
          f, c);
-    if (lane == 0) {
-      o[0] = (float)sm.t[0]; o[1] = (float)sm.t[1]; o[2] = (float)sm.t[2];
-      if (inl_out) inl_out[h] = (int32_t)use;
-    }
+    if (lane == 0) store_epnp(sm, jh, ph, focal, img_size, o, inl_out ? inl_out + h : nullptr, use);
     return;
   }
   // this lane's point for the inlier test
@@ -627,10 +645,7 @@ cam_trans_pnp_kernel(const float* __restrict__ j3d, const float* __restrict__ pj
   epnp(sm, lane, best, hf ? fX : 0.f, hf ? fY : 0.f, hf ? fZ : 0.f, hf ? pix_fp64_normalised(fu, f, c) : 0.0,
        hf ? pix_fp64_normalised(fv, f, c) : 0.0, f, c);
   const unsigned joints = __reduce_or_sync(FULL, (mine && inl_me) ? 1u << sm.idx[lane] : 0u);
-  if (lane == 0) {
-    o[0] = (float)sm.t[0]; o[1] = (float)sm.t[1]; o[2] = (float)sm.t[2];
-    if (inl_out) inl_out[h] = (int32_t)joints;
-  }
+  if (lane == 0) store_epnp(sm, jh, ph, focal, img_size, o, inl_out ? inl_out + h : nullptr, joints);
 }
 
 }  // namespace
