@@ -42,6 +42,7 @@ _DEFAULTS = dict(
     track_hands=False, track_gate=8, track_max_missed=15,  # multi-hand tracking in process_results (DESIGN.md): track ids,
                                                           # and with temporal_optimization one filter bank per track;
                                                           # gate in centre-map cells, max_missed in frames
+    track_streams=1,                                       # streams one batch may hold (batch_forward's stream_ids)
     model_path=os.path.join(project_dir, "checkpoints", "wild.pkl"),
     mano_root=os.path.join(project_dir, "mano"),           # acr/mano_wrapper.py:22 uses 'mano/'
     cam_trans_mode="lstsq",                                # 'lstsq' (device least squares, SURVEY 8f-1) | 'pnp' (device

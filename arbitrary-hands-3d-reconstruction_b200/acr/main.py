@@ -24,6 +24,37 @@ def _check_tracker(tracker, K):
         raise ValueError(f"this tracker is built for K={tracker.K}, but max_hands_per_side is {K}")
 
 
+def _stream_buffers(tracker, batch, dev):
+    """Static (B,) int32 stream ids and begin flags of a graph captured with a multi-stream tracker, else None."""
+    if tracker is None or tracker.streams == 1:
+        return None
+    return (torch.zeros(batch, dtype=torch.int32, device=dev), torch.zeros(batch, dtype=torch.int32, device=dev))
+
+
+def _load_streams(static, stream_ids, stream_begin):
+    """Check a replay's stream ids / begin flags (before anything is enqueued), then copy them into the graph's."""
+    sid, sbeg = static
+    for name, v in (("stream_ids", stream_ids), ("stream_begin", stream_begin)):
+        if v is not None and tuple(torch.as_tensor(v).shape) != tuple(sid.shape):
+            raise ValueError(f"{name} must have shape {tuple(sid.shape)}, got {tuple(torch.as_tensor(v).shape)}")
+    if stream_ids is None:
+        raise ValueError("this graph tracks several streams: replay needs stream_ids, the stream slot of each frame")
+    sid.copy_(torch.as_tensor(stream_ids), non_blocking=True)
+    if stream_begin is None:
+        sbeg.zero_()
+    else:
+        sbeg.copy_(torch.as_tensor(stream_begin), non_blocking=True)
+
+
+def _device_ints(v, B, dev, name):
+    if v is None:
+        return None
+    t = torch.as_tensor(v)
+    if tuple(t.shape) != (B,):
+        raise ValueError(f"{name} must have shape ({B},), got {tuple(t.shape)}")
+    return t.to(device=dev, dtype=torch.int32).contiguous()
+
+
 class ACR(nn.Module):
     def __init__(self, args_set=None, state_dict=None, mano_assets=None):
         super().__init__()
@@ -43,34 +74,55 @@ class ACR(nn.Module):
         self.mano_regression = MANOWrapper(mano_assets).cuda()
 
     def _track_results(self, outputs):
-        """``track_hands``: the rows of this batch (B consecutive frames of one stream) through the device tracker,
-        which also filters poses / betas per track when ``temporal_optimization`` is on; sets outputs['track_id']."""
+        """``track_hands``: the rows of this batch through the device tracker, which also filters poses / betas per
+        track when ``temporal_optimization`` is on; sets outputs['track_id'].  With ``track_streams`` = 1 the batch
+        is B consecutive frames of one stream; with more, meta_data['stream_ids'] gives each image's stream slot
+        (batch_forward's ``stream_ids``), the frames of a stream in batch order, and a track is keyed by (stream,
+        id)."""
         from acr.result_parser import ResultParser
         from acr_b200 import ops as _ops
         K = ResultParser.hands_per_side()
-        bids = outputs['meta_data'].get('batch_ids')
+        S = int(getattr(self, 'track_streams', 1))
+        meta = outputs['meta_data']
+        bids = meta.get('batch_ids')
         if bids is None:
             raise ValueError("track_hands needs meta_data['batch_ids'] (batch_forward sets arange(B))")
         bids = torch.as_tensor(bids).flatten().cpu()
         B = int(bids.numel())
-        if not torch.equal(bids, torch.arange(B, dtype=bids.dtype)):
-            raise ValueError("track_hands treats the batch as consecutive frames of one stream: batch_ids must be "
-                             "arange(B)")
-        smooth = float(self.smooth_coeff) if getattr(self, 'temporal_optimization', False) else None
-        cfg = (K, int(self.track_gate), int(self.track_max_missed), smooth)
-        t = getattr(self, '_hand_tracker', None)
-        if t is None or (t.K, t.gate, t.max_missed, t.smooth_coeff) != cfg:     # new settings start new tracks
-            t = self._hand_tracker = _ops.HandTracker(outputs['params_dict']['poses'].device, *cfg)
         pd = outputs['params_dict']
-        n = pd['poses'].shape[0]
         dev = pd['poses'].device
+        img = outputs['reorganize_idx']
+        sid = sbeg = None
+        if S == 1:
+            if not torch.equal(bids, torch.arange(B, dtype=bids.dtype)):
+                raise ValueError("track_hands treats the batch as consecutive frames of one stream: batch_ids must be "
+                                 "arange(B)")
+        else:
+            if meta.get('stream_ids') is None:
+                raise ValueError(f"track_streams={S}: track_hands needs meta_data['stream_ids'] (batch_forward's "
+                                 "stream_ids), the stream slot of each image")
+            if torch.unique(bids).numel() != B:
+                raise ValueError("track_hands with several streams needs distinct batch_ids, one per image")
+            # the rows carry batch ids; the tracker wants each row's position in the batch
+            pos = torch.full((int(bids.max()) + 1,), -1, dtype=torch.int64)
+            pos[bids.long()] = torch.arange(B)
+            img = pos.to(dev)[torch.as_tensor(img, device=dev).long()]
+            sid = _device_ints(meta['stream_ids'], B, dev, 'stream_ids')
+            sbeg = _device_ints(meta.get('stream_begin'), B, dev, 'stream_begin')
+        smooth = float(self.smooth_coeff) if getattr(self, 'temporal_optimization', False) else None
+        cfg = (K, int(self.track_gate), int(self.track_max_missed), smooth, S)
+        t = getattr(self, '_hand_tracker', None)
+        if t is None or (t.K, t.gate, t.max_missed, t.smooth_coeff, t.streams) != cfg:  # new settings: new tracks
+            t = self._hand_tracker = _ops.HandTracker(dev, *cfg)
+        n = pd['poses'].shape[0]
         cen = torch.cat([outputs['l_centers_pred'], outputs['r_centers_pred']]).to(dev)     # (x, y) per row
         i32 = lambda v: v.to(device=dev, dtype=torch.int32)
-        row_src = torch.stack([i32(outputs['reorganize_idx']), i32(outputs['output_hand_type']),
+        row_src = torch.stack([i32(img), i32(outputs['output_hand_type']),
                                i32(cen[:, 1] * 64 + cen[:, 0]), torch.zeros(n, dtype=torch.int32, device=dev)],
                               1).contiguous()
         poses, betas = pd['poses'].contiguous(), pd['betas'].contiguous()
-        ids = _ops.track_rows(t, B, row_src, outputs['detection_flag'].float().contiguous(), poses, betas)
+        ids = _ops.track_rows(t, B, row_src, outputs['detection_flag'].float().contiguous(), poses, betas,
+                              frame_stream=sid, frame_begin=sbeg)
         pd['poses'], pd['betas'] = poses, betas
         outputs['track_id'] = ids[:n].clone()
 
@@ -98,32 +150,48 @@ class ACR(nn.Module):
         return outputs
 
     @torch.no_grad()
-    def batch_forward(self, images_rgb_u8, offsets=None, batch_ids=None):
-        """B frames (uint8 BHWC RGB, already 512x512) -> reference-schema outputs incl. MANO."""
+    def batch_forward(self, images_rgb_u8, offsets=None, batch_ids=None, stream_ids=None, stream_begin=None):
+        """B frames (uint8 BHWC RGB, already 512x512) -> reference-schema outputs incl. MANO.  ``stream_ids`` /
+        ``stream_begin`` (B,): each image's stream slot and start-over flag for ``track_hands`` with
+        ``track_streams`` > 1 (meta_data['stream_ids'] / ['stream_begin'])."""
         B = images_rgb_u8.shape[0]
         if offsets is None:
             offsets = torch.tensor([[512., 512, 0, 0, 0, 0, 0, 0, 0, 0]]).repeat(B, 1)
         meta = {'image': images_rgb_u8, 'offsets': offsets,
                 'batch_ids': torch.arange(B) if batch_ids is None else batch_ids}
+        if stream_ids is not None:
+            meta['stream_ids'] = stream_ids
+        if stream_begin is not None:
+            meta['stream_begin'] = stream_begin
         outputs = self.model(meta, **self.demo_cfg)
         return self.process_results(outputs)
 
     @torch.no_grad()
-    def fused_forward(self, images_rgb_u8, offsets, out=None, peers=None, tracker=None):
+    def fused_forward(self, images_rgb_u8, offsets, out=None, peers=None, tracker=None, stream_ids=None,
+                      stream_begin=None):
         """Sync-free pipeline: backbone + heads + parse + MANO enqueued back to back; MANO runs over
         the worst case 2KB rows (K = ``max_hands_per_side``) and skips rows >= L+R on the device.  Returns dense
         buffers (zero copy: the parse buffers are shared per batch size, consume them before the next call).  ``peers``
         (acr_b200.dist.PeerVertexGather): the MANO kernel also stores vertices and row counts into every
         rank's gather buffer.  ``tracker`` (acr_b200.ops.HandTracker): the batch is B consecutive frames of one
         stream, tracked (and, with the tracker's smooth_coeff, filtered per track) between parse and MANO;
-        mano['track_id'] is the tracker's id buffer."""
+        mano['track_id'] is the tracker's id buffer.  With a multi-stream tracker (``streams`` > 1), ``stream_ids``
+        (B,) int gives each image's stream slot (the frames of one stream in batch order) and ``stream_begin`` (B,)
+        starts a slot over at each nonzero frame; a row's stream is ``stream_ids[reorganize_idx]``."""
         if tracker is not None and peers is not None:
             raise ValueError("a tracker follows one stream: it cannot be combined with a cross-rank vertex gather")
+        if tracker is None and (stream_ids is not None or stream_begin is not None):
+            raise ValueError("stream_ids / stream_begin need a tracker")
         B = images_rgb_u8.shape[0]
+        dev = images_rgb_u8.device
+        sid = _device_ints(stream_ids, B, dev, 'stream_ids')
+        sbeg = _device_ints(stream_begin, B, dev, 'stream_begin')
+        if tracker is not None and tracker.streams > 1 and sid is None:
+            raise ValueError(f"this tracker follows {tracker.streams} streams: give stream_ids, the slot of each frame")
         meta = {'image': images_rgb_u8, 'offsets': offsets, 'batch_ids': None}
         eng, bufs = self.model.forward_dense(meta)
         from acr_b200 import ops as _ops
-        ids = _ops.track_hands(bufs, tracker) if tracker is not None else None
+        ids = _ops.track_hands(bufs, tracker, sid, sbeg) if tracker is not None else None
         ml, mr = self.mano_regression.models()
         mano = _ops.mano_forward(ml, mr, bufs.poses, bufs.betas, bufs.hand_type, 1, self.mano_regression.center_idx,
                                  bufs.cam, bufs.offsets_out, n_dev=bufs.counts[2:3], peers=peers, counts=bufs.counts)
@@ -142,7 +210,9 @@ class ACR(nn.Module):
         frame-by-frame video / webcam loop (acr/main.py:183-201, batch 1) latency-bound by the GPU instead
         of by ~380 host-side launches.  The graph is bound to the ``max_hands_per_side`` it was captured with
         (``replay.hands_per_side``); a replay under another value raises.  With a ``tracker`` the graph also tracks:
-        each replay continues the tracker's state from the previous one (``tracker.reset()`` starts over)."""
+        each replay continues the tracker's state from the previous one (``tracker.reset()`` starts over).  With a
+        multi-stream tracker the replay is ``replay(frames_u8, offsets, stream_ids, stream_begin=None)``: (B,) stream
+        slots and start-over flags per frame, copied into static buffers of the graph."""
         from acr.result_parser import ResultParser
         K = ResultParser.hands_per_side()
         _check_tracker(tracker, K)
@@ -156,20 +226,34 @@ class ACR(nn.Module):
                 self.fused_forward(frames, offsets)         # (without the tracker: its state stays as it is)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
+        streams = _stream_buffers(tracker, batch, dev)
         if tracker is not None:
             tracker.ids(batch)                              # the id buffer exists before the capture
+            if streams is not None:
+                tracker.workspace(batch)                    # and the workspace
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            bufs, mano = self.fused_forward(frames, offsets, tracker=tracker)
+            bufs, mano = self.fused_forward(frames, offsets, tracker=tracker, stream_ids=streams and streams[0],
+                                            stream_begin=streams and streams[1])
 
-        def replay(frames_u8, offs):
+        def replay_one(frames_u8, offs):
             _check_hands_per_side(K)
             frames.copy_(frames_u8, non_blocking=True)
             offsets.copy_(offs, non_blocking=True)
             graph.replay()
             return bufs, mano
 
+        def replay_streams(frames_u8, offs, stream_ids=None, stream_begin=None):
+            _check_hands_per_side(K)
+            _load_streams(streams, stream_ids, stream_begin)
+            frames.copy_(frames_u8, non_blocking=True)
+            offsets.copy_(offs, non_blocking=True)
+            graph.replay()
+            return bufs, mano
+
+        replay = replay_one if streams is None else replay_streams
         replay.graph, replay.static_inputs, replay.hands_per_side = graph, (frames, offsets), K
+        replay.static_streams = streams
         return replay
 
     @torch.no_grad()
@@ -179,7 +263,8 @@ class ACR(nn.Module):
         ``replay(frames) -> (bufs, mano)`` for a list of exactly ``batch`` BGR frames (numpy arrays, CPU or CUDA
         tensors) of any sizes, each replay its own, whose packed H*W*3 bytes sum to at most ``max_frame_bytes``.  Host
         frames travel in one H2D copy; a list that does not fit raises before anything is enqueued.  Like
-        ``capture_graph``, the graph is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it."""
+        ``capture_graph``, the graph is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with
+        a multi-stream tracker the replay is ``replay(frames, stream_ids, stream_begin=None)``."""
         from acr.result_parser import ResultParser
         from acr_b200.preprocess import RaggedFrames
         K = ResultParser.hands_per_side()
@@ -196,19 +281,34 @@ class ACR(nn.Module):
                 self.fused_forward(*rf.launch())
         cur.wait_stream(side)
         torch.cuda.synchronize(dev)
+        streams = _stream_buffers(tracker, batch, dev)
         if tracker is not None:
             tracker.ids(batch)
+            if streams is not None:
+                tracker.workspace(batch)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker)
+            bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker, stream_ids=streams and streams[0],
+                                            stream_begin=streams and streams[1])
 
-        def replay(frames):
+        def replay_one(frames):
             _check_hands_per_side(K)
             rf.load(frames)
             graph.replay()
             return bufs, mano
 
+        def replay_streams(frames, stream_ids=None, stream_begin=None):
+            _check_hands_per_side(K)
+            if len(frames) != batch:                        # RaggedFrames checks it too, but after the stream ids
+                raise ValueError(f"this graph takes exactly {batch} frames, got {len(frames)}")
+            _load_streams(streams, stream_ids, stream_begin)
+            rf.load(frames)
+            graph.replay()
+            return bufs, mano
+
+        replay = replay_one if streams is None else replay_streams
         replay.graph, replay.frames, replay.hands_per_side = graph, rf, K
+        replay.static_streams = streams
         return replay
 
     @torch.no_grad()

@@ -242,24 +242,31 @@ def one_euro_smooth(poses: torch.Tensor, betas: torch.Tensor, state: OneEuroStat
 
 
 class HandTracker:
-    """Device-side state of multi-hand tracking for one stream (acr_b200_track_hands): K track slots per side, each
-    with its id, last cell, missed-frame count and OneEuro bank.  ``gate`` is in centre-map cells (8 cells = 64 px
-    on the 512 input; >= 90 never rejects), ``max_missed`` in frames (15 = half a second at 30 fps);
-    ``smooth_coeff`` None tracks ids only, a positive value also filters poses and betas per track.  Owns one (2KB,)
-    int32 id buffer per batch size, reused by every call (zero copy, like ParseBuffers)."""
+    """Device-side state of multi-hand tracking (acr_b200_track_hands): K track slots per side, each with its id, last
+    cell, missed-frame count and OneEuro bank, for one stream or, with ``streams`` = S > 1, for S streams whose frames
+    share a batch (acr_b200_track_streams; every call then says which stream each image belongs to).  ``gate`` is in
+    centre-map cells (8 cells = 64 px on the 512 input; >= 90 never rejects), ``max_missed`` in frames (15 = half a
+    second at 30 fps); ``smooth_coeff`` None tracks ids only, a positive value also filters poses and betas per track.
+    ``state`` is S consecutive slots of acr_b200_track_state_bytes(K) bytes, slot s byte for byte a single-stream
+    tracker's state.  Owns one (2KB,) int32 id buffer (and, for several streams, one workspace) per batch size, reused
+    by every call (zero copy, like ParseBuffers)."""
 
-    def __init__(self, device, K: int, gate: int = 8, max_missed: int = 15, smooth_coeff: Optional[float] = 4.0):
+    def __init__(self, device, K: int, gate: int = 8, max_missed: int = 15, smooth_coeff: Optional[float] = 4.0,
+                 streams: int = 1):
         if not 1 <= int(K) <= MAX_HANDS_PER_SIDE:
             raise ValueError(f"hands per side must be in 1..{MAX_HANDS_PER_SIDE}, got {K}")
         if int(gate) < 0 or int(max_missed) < 0:
             raise ValueError(f"gate and max_missed must be >= 0, got {gate}, {max_missed}")
         if smooth_coeff is not None and not float(smooth_coeff) > 0:
             raise ValueError(f"smooth_coeff must be positive or None, got {smooth_coeff}")
+        if not 1 <= int(streams) <= MAX_TRACK_STREAMS:
+            raise ValueError(f"streams must be in 1..{MAX_TRACK_STREAMS}, got {streams}")
         self.device, self.K, self.gate, self.max_missed = torch.device(device), int(K), int(gate), int(max_missed)
         self.smooth_coeff = None if smooth_coeff is None else float(smooth_coeff)
-        self.state = torch.zeros(int(L.load().acr_b200_track_state_bytes(self.K)), dtype=torch.uint8,
-                                 device=self.device)
-        self._ids = {}
+        self.streams = int(streams)
+        self.slot_bytes = int(L.load().acr_b200_track_state_bytes(self.K))
+        self.state = torch.zeros(self.streams * self.slot_bytes, dtype=torch.uint8, device=self.device)
+        self._ids, self._ws = {}, {}
 
     def ids(self, B: int) -> torch.Tensor:
         """The (2KB,) id buffer of batch size B."""
@@ -267,18 +274,43 @@ class HandTracker:
             self._ids[B] = torch.full((2 * self.K * B,), -1, dtype=torch.int32, device=self.device)
         return self._ids[B]
 
+    def workspace(self, B: int) -> torch.Tensor:
+        """The device scratch of acr_b200_track_streams at batch size B (2KB rows)."""
+        if B not in self._ws:
+            nb = int(L.load().acr_b200_track_streams_workspace_bytes(2 * self.K * B, int(B), self.streams))
+            self._ws[B] = torch.empty(nb, dtype=torch.uint8, device=self.device)
+        return self._ws[B]
+
+    def slot(self, s: int) -> torch.Tensor:
+        """Stream s's state (a view): byte for byte the state of a single-stream tracker after the same frames."""
+        return self.state[s * self.slot_bytes:(s + 1) * self.slot_bytes]
+
     def reset(self) -> None:
-        """No tracks, birth counters at zero; in place, so a captured graph stays valid."""
+        """No tracks, birth counters at zero, in every stream; in place, so a captured graph stays valid."""
         self.state.zero_()
+
+
+def _frame_ints(t: Optional[torch.Tensor], B: int, name: str) -> Optional[torch.Tensor]:
+    if t is None:
+        return None
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.int32 and t.is_contiguous()
+            and tuple(t.shape) == (B,)):
+        raise ValueError(f"{name} must be a contiguous ({B},) int32 CUDA tensor")
+    return t
 
 
 def track_rows(tracker: HandTracker, B: int, row_src: torch.Tensor, detection_flag: Optional[torch.Tensor],
                poses: Optional[torch.Tensor] = None, betas: Optional[torch.Tensor] = None,
-               n_dev: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Track the rows of B consecutive frames (``row_src`` (n,4) int32 in the parse's layout, n <= 2KB) on the current
-    stream, no host sync.  With the tracker's ``smooth_coeff`` set, ``poses`` (n,48) and ``betas`` (n,10) (contiguous
-    fp32) are filtered in place.  Returns the tracker's id buffer for B; rows [0, min(n, n_dev)) are valid."""
-    dev = L.require_cuda(row_src, detection_flag, poses, betas, n_dev, tracker.state)
+               n_dev: Optional[torch.Tensor] = None, frame_stream: Optional[torch.Tensor] = None,
+               frame_begin: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Track the rows of a batch of B images (``row_src`` (n,4) int32 in the parse's layout, n <= 2KB) on the current
+    stream, no host sync.  With one stream the images are B consecutive frames.  ``frame_stream`` (B,) int32 on the
+    device gives each image's stream slot in 0..streams-1 (a multi-stream tracker needs it; another value leaves the
+    image's rows untracked), the frames of one stream in ascending batch index; ``frame_begin`` (B,) int32 starts a
+    stream over (zeroed slot) at each nonzero frame.  With the tracker's ``smooth_coeff`` set, ``poses`` (n,48) and
+    ``betas`` (n,10) (contiguous fp32) are filtered in place.  Returns the tracker's id buffer for B; rows
+    [0, min(n, n_dev)) are valid."""
+    dev = L.require_cuda(row_src, detection_flag, poses, betas, n_dev, frame_stream, frame_begin, tracker.state)
     n = row_src.shape[0]
     assert row_src.dtype == torch.int32 and row_src.is_contiguous() and row_src.shape[1:] == (4,)
     assert detection_flag is None or (detection_flag.dtype == torch.float32 and detection_flag.is_contiguous())
@@ -286,24 +318,41 @@ def track_rows(tracker: HandTracker, B: int, row_src: torch.Tensor, detection_fl
     if smooth:
         assert poses is not None and betas is not None, "a smoothing tracker needs poses and betas"
         assert poses.is_contiguous() and betas.is_contiguous() and poses.dtype == betas.dtype == torch.float32
+    frame_stream = _frame_ints(frame_stream, int(B), "frame_stream")
+    frame_begin = _frame_ints(frame_begin, int(B), "frame_begin")
+    if frame_stream is None and tracker.streams > 1:
+        raise ValueError(f"this tracker follows {tracker.streams} streams: give frame_stream, the stream of each image")
+    if frame_stream is None and frame_begin is not None:
+        frame_stream = torch.zeros(int(B), dtype=torch.int32, device=dev)
     ids = tracker.ids(B)
+    P = lambda t: L.ptr(t) if smooth else None
     with L.on(dev):
-        L.check(L.load().acr_b200_track_hands(L.ptr(poses) if smooth else None, L.ptr(betas) if smooth else None,
-                                              L.ptr(row_src), L.ptr(detection_flag), L.ptr(n_dev), n, int(B),
-                                              tracker.K, tracker.gate, tracker.max_missed,
-                                              tracker.smooth_coeff or 0.0, L.ptr(tracker.state), L.ptr(ids),
-                                              L.current_stream(dev)), "track_hands")
+        if frame_stream is None:
+            L.check(L.load().acr_b200_track_hands(P(poses), P(betas), L.ptr(row_src), L.ptr(detection_flag),
+                                                  L.ptr(n_dev), n, int(B), tracker.K, tracker.gate, tracker.max_missed,
+                                                  tracker.smooth_coeff or 0.0, L.ptr(tracker.state), L.ptr(ids),
+                                                  L.current_stream(dev)), "track_hands")
+        else:
+            L.check(L.load().acr_b200_track_streams(P(poses), P(betas), L.ptr(row_src), L.ptr(detection_flag),
+                                                    L.ptr(n_dev), n, int(B), tracker.K, tracker.gate,
+                                                    tracker.max_missed, tracker.smooth_coeff or 0.0,
+                                                    L.ptr(tracker.state), L.ptr(ids), L.ptr(frame_stream),
+                                                    L.ptr(frame_begin), tracker.streams,
+                                                    L.ptr(tracker.workspace(int(B))), L.current_stream(dev)),
+                    "track_streams")
     return ids
 
 
-def track_hands(bufs: "ParseBuffers", tracker: HandTracker) -> torch.Tensor:
-    """Track the hands of a parse (ParseBuffers of B consecutive frames of one stream) on the current stream, no host
-    sync: poses / betas are filtered in place when the tracker smooths (params_pred, global_orient and hand_pose stay
-    raw).  Returns the tracker's (2KB,) int32 id buffer, valid over rows [0, counts[2])."""
+def track_hands(bufs: "ParseBuffers", tracker: HandTracker, frame_stream: Optional[torch.Tensor] = None,
+                frame_begin: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Track the hands of a parse (ParseBuffers of B frames: consecutive frames of one stream, or with
+    ``frame_stream`` / ``frame_begin`` as in track_rows, frames of several) on the current stream, no host sync:
+    poses / betas are filtered in place when the tracker smooths (params_pred, global_orient and hand_pose stay raw).
+    Returns the tracker's (2KB,) int32 id buffer, valid over rows [0, counts[2])."""
     if tracker.K != bufs.K:
         raise ValueError(f"this tracker is built for K={tracker.K}, the parse buffers for K={bufs.K}")
     return track_rows(tracker, bufs.B, bufs.row_src, bufs.detection_flag, bufs.poses, bufs.betas,
-                      n_dev=bufs.counts[2:3])
+                      n_dev=bufs.counts[2:3], frame_stream=frame_stream, frame_begin=frame_begin)
 
 
 # ------------------------------------------------------------------------------ rotations
@@ -332,6 +381,7 @@ def rodrigues(aa: torch.Tensor) -> torch.Tensor:
 
 # --------------------------------------------------------------------------------- parse
 MAX_HANDS_PER_SIDE = 16
+MAX_TRACK_STREAMS = 4096            # acr_b200_track_streams' S
 
 
 class ParseBuffers:

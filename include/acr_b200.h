@@ -259,6 +259,28 @@ int acr_b200_track_hands(float* poses, float* betas, const int32_t* row_src, con
                          const int32_t* n_dev, int n_max, int B, int K, int gate, int max_missed, float smooth_coeff,
                          void* state, int32_t* track_id, void* stream);
 
+/* Multi-hand tracking of up to S streams in one batch: acr_b200_track_hands per stream, with the streams' frames
+ * interleaved in any way.  frame_stream (B) int32 on the device gives the stream slot of each image, in 0..S-1; the
+ * images of one stream are its frames in time order, in ascending batch index.  For every stream s the result is
+ * acr_b200_track_hands run on s's frames alone, bit for bit: the rows of s's images in their table order, the images
+ * renumbered 0..B_s-1 in batch order, and slot s of the state.  So each rule of the single-stream call (detections,
+ * malformed, out-of-range and out-of-time-order rows, ids 2*c + side with a birth counter per stream and side)
+ * applies per stream, and the key of a track is (stream, id).  A frame whose stream is outside 0..S-1 is not tracked:
+ * its rows get id -1 and stay untouched.  frame_begin (B) int32 on the device, or NULL: a nonzero entry zeroes the
+ * frame's stream slot just before that frame, as a zeroed single-stream state (a new camera in that slot); which
+ * rows are detections is still decided over the stream's rows of the whole call, as one single-stream call does.
+ * `state`: S consecutive slots of acr_b200_track_state_bytes(K) bytes; slot s is byte for byte a single-stream state,
+ * so one can be copied in or out as it is.  `workspace`: acr_b200_track_streams_workspace_bytes(n_max, B, S) bytes of
+ * caller-owned device scratch (the per-stream bucketing of frames and rows).  The launches depend on B, K and S only:
+ * no host sync, capturable in a CUDA graph.  The checks of acr_b200_track_hands, S outside 1..4096, or a NULL
+ * frame_stream or workspace is ACR_B200_EINVAL and nothing is launched.  The workspace size is 0 for n_max < 0, B < 1
+ * or S outside 1..4096.  tests/stream_track_ref.py is the statement.                                           */
+size_t acr_b200_track_streams_workspace_bytes(int n_max, int B, int S);
+int acr_b200_track_streams(float* poses, float* betas, const int32_t* row_src, const float* detection_flag,
+                           const int32_t* n_dev, int n_max, int B, int K, int gate, int max_missed, float smooth_coeff,
+                           void* state, int32_t* track_id, const int32_t* frame_stream, const int32_t* frame_begin,
+                           int S, void* workspace, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Rotations
  * ---------------------------------------------------------------------------------------- */
