@@ -131,7 +131,8 @@ class ACR(nn.Module):
         if getattr(self, 'track_hands', False):
             self._track_results(outputs)
         # temporal optimisation (acr/main.py:69-83): OneEuro filters on poses / betas, one bank per hand type,
-        # applied between parse and MANO -- here one device kernel instead of host-side filter objects
+        # applied between parse and MANO -- here the device tracker at K = 1 with the gate open and no miss limit,
+        # whose one track per side is that bank
         elif getattr(self, 'temporal_optimization', False):
             from acr.result_parser import ResultParser
             if ResultParser.hands_per_side() > 1:
@@ -140,11 +141,15 @@ class ACR(nn.Module):
             from acr_b200 import ops as _ops
             pd = outputs['params_dict']
             assert len(pd['poses']) == 2, 'temporal smoothing streams one frame (two hand slots) at a time'
+            dev = pd['poses'].device
             if getattr(self, '_one_euro', None) is None:
-                self._one_euro = _ops.OneEuroState(pd['poses'].device)
+                self._one_euro = _ops.HandTracker(dev, 1, _ops.TRACK_GATE_OPEN, _ops.TRACK_NO_MISS_LIMIT)
+            self._one_euro.smooth_coeff = float(self.smooth_coeff)     # read per call; the history stays
+            row_src = torch.zeros(2, 4, dtype=torch.int32, device=dev)  # one frame; any cell, as the gate is open
+            row_src[:, 1] = outputs['output_hand_type']
             poses, betas = pd['poses'].contiguous(), pd['betas'].contiguous()
-            _ops.one_euro_smooth(poses, betas, self._one_euro, float(self.smooth_coeff),
-                                 hand_type=outputs['output_hand_type'], detection_flag=outputs['detection_flag_cache'].float())
+            _ops.track_rows(self._one_euro, 1, row_src, outputs['detection_flag_cache'].float().contiguous(), poses,
+                            betas)
             pd['poses'], pd['betas'] = poses, betas
         outputs = self.mano_regression(outputs, outputs['meta_data'])
         return outputs

@@ -214,31 +214,9 @@ def cam_trans_mode(mode: str, j3d: torch.Tensor, pj2d: torch.Tensor, focal_lengt
     return None
 
 
-class OneEuroState:
-    """Device-side history of the temporal filter (one bank per hand type); zero = no history."""
-
-    def __init__(self, device):
-        self.state = torch.zeros(int(L.load().acr_b200_one_euro_state_floats()), device=device)
-
-    def reset(self) -> None:
-        self.state.zero_()
-
-
-def one_euro_smooth(poses: torch.Tensor, betas: torch.Tensor, state: OneEuroState, smooth_coeff: float = 4.0,
-                    hand_type: Optional[torch.Tensor] = None, detection_flag: Optional[torch.Tensor] = None,
-                    n_dev: Optional[torch.Tensor] = None) -> None:
-    """In-place temporal smoothing of (n,48) poses and (n,10) betas (drop-in for acr.utils.smooth_results
-    applied per hand as in acr/main.py:69-83).  The state has one bank per hand type, so at most two rows (one per
-    type; row r uses bank r without ``hand_type``): more raise AcrB200Error, like the C entry point."""
-    dev = L.require_cuda(poses, betas, hand_type, detection_flag, n_dev, state.state)
-    assert poses.is_contiguous() and betas.is_contiguous() and poses.dtype == betas.dtype == torch.float32
-    if poses.shape[0] > 2:
-        raise L.AcrB200Error(f"one_euro_smooth: at most 2 rows, one per hand type (got {poses.shape[0]})")
-    if poses.shape[0]:
-        with L.on(dev):
-            L.check(L.load().acr_b200_one_euro_smooth(L.ptr(poses), L.ptr(betas), L.ptr(hand_type), L.ptr(detection_flag),
-                                                      L.ptr(n_dev), poses.shape[0], L.ptr(state.state), float(smooth_coeff),
-                                                      L.current_stream(dev)), "one_euro_smooth")
+# K = 1 with the gate open and no miss limit is the reference's per-hand-type OneEuro smoothing (one bank per side)
+TRACK_GATE_OPEN = 90                # cells: 63^2 + 63^2 < 90^2, so no pair on the 64x64 map is out of the gate
+TRACK_NO_MISS_LIMIT = 2 ** 31 - 1   # frames: a track is never ended for missing frames
 
 
 class HandTracker:

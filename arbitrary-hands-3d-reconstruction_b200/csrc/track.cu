@@ -5,7 +5,7 @@
 //
 // One CTA per (stream, side); the state is per stream and side: a header (birth counter), K slot records (id, cell, missed, live) and K
 // banks of 3 x 64 floats (previous raw value, filtered value, filtered derivative of the 45 pose values, 10 betas
-// and 9 root-matrix entries, acr_b200_one_euro_smooth's layout).  Frames go in chunks of TR_CHUNK:
+// and 9 root-matrix entries: the quantities of the reference's smooth_results).  Frames go in chunks of TR_CHUNK:
 //   association  warp 0 walks the row table in windows of 32 rows (coalesced), keeps a side's rows whose images
 //                do not go back in time, and runs match / miss / birth per frame with the K slots in lanes 0..K-1
 //                and the frame's detections in lanes 0..nd-1; the match takes the smallest packed key
@@ -22,7 +22,6 @@
 // thread in a fixed order, so repeated launches are bit-identical and one launch over B frames equals B launches of
 // one frame.
 #include "common.cuh"
-#include "one_euro.cuh"
 #include "rotation.cuh"
 
 namespace acr {
@@ -44,6 +43,27 @@ __host__ __device__ constexpr size_t track_side_bytes(int K) {
   return 16 + (size_t)K * sizeof(TrackSlot) + (size_t)K * 3 * TR_ELEMS * sizeof(float);
 }
 
+// One step of the OneEuro filter (acr/utils.py:1485-1527) on one bank element:
+//   x_hat = lowpass(x, alpha(mincutoff + beta*|lowpass(dx, alpha(dcutoff))|)),  dx = (x - x_prev)*freq,
+//   alpha(c) = 1 / (1 + (1/(2 pi c)) / (1/freq)),  freq = 30 (te = 1/30 whatever the gap), beta = 0.7, dcutoff = 1.
+__device__ __forceinline__ float one_euro_alpha(float cutoff) {
+  const float te = 1.0f / 30.0f;
+  const float tau = 1.0f / (2.0f * 3.14159265358979323846f * cutoff);
+  return 1.0f / (1.0f + tau / te);
+}
+
+// x: the new raw value; raw, filt, fdx: the bank's previous raw value, filtered value and filtered derivative.
+// Writes the filtered value xh and the filtered derivative edx.  The roundings are spelled out (which product each
+// FMA absorbs), so the result does not depend on how the compiler contracts the surrounding code.
+__device__ __forceinline__ void one_euro_step(float x, float mincut, float raw, float filt, float fdx, float& xh,
+                                              float& edx) {
+  const float dx = __fmul_rn(__fsub_rn(x, raw), 30.0f);
+  const float ad = one_euro_alpha(1.0f);
+  edx = __fmaf_rn(fdx, 1.0f - ad, __fmul_rn(dx, ad));
+  const float a = one_euro_alpha(__fmaf_rn(fabsf(edx), 0.7f, mincut));
+  xh = __fmaf_rn(a, x, __fmul_rn(1.0f - a, filt));
+}
+
 template <bool kPiTrig>
 __device__ __forceinline__ float rodrigues_entry(float ax, float ay, float az, int j) {
   float R[9];
@@ -55,7 +75,7 @@ __device__ __forceinline__ float rodrigues_entry(float ax, float ay, float az, i
   return x;
 }
 
-// Entry j of rodrigues() as acr_b200_one_euro_smooth evaluates it (sincosf).  sincosf's reduction for |angle / 2|
+// Entry j of rodrigues() in its default sincosf form.  sincosf's reduction for |angle / 2|
 // >= 105615 keeps a scratch array in local memory; such angles (beyond 2e5 rad) take the sincospif form instead,
 // which needs none.  The test is sincosf's own, so the compiler drops that reduction from the first branch.
 __device__ __forceinline__ float track_rodrigues_entry(float ax, float ay, float az, int j) {

@@ -226,21 +226,11 @@ int acr_b200_preprocess_ragged(const uint8_t* frames_bgr, int64_t src_bytes, con
                                const int16_t* coef, const int32_t* ofs, int out_size, uint8_t* out_rgb,
                                float* offsets, void* stream);
 
-/* Temporal OneEuro smoothing of poses / betas between parse and MANO, in place, on the device
- * (SURVEY.md 8f-3).  Replaces OneEuroFilter / LowPassFilter (acr/utils.py:1485-1527), smooth_results
- * (:1478-1482), smooth_global_rot_matrix (:1466-1470) and the per-frame host loop of acr/main.py:69-83.
- * `state`: device buffer of acr_b200_one_euro_state_floats() floats, zero-initialised = "no history";
- * one filter bank per hand type (0 left, 1 right), like the reference's filter_dict -- i.e. for streaming
- * one frame at a time (the reference asserts exactly two rows).  Rows with detection_flag == 0 are skipped.
- * poses (n,48) and betas (n,10) are updated in place.
- * Row r uses bank hand_type[r], or bank r when hand_type is NULL; the two rows of a call must use different banks.
- * The state holds two banks, so n_max > 2 is ACR_B200_EINVAL and nothing is launched.                */
-size_t acr_b200_one_euro_state_floats(void);
-int acr_b200_one_euro_smooth(float* poses, float* betas, const int32_t* hand_type, const float* detection_flag,
-                             const int32_t* n_dev, int n_max, float* state, float smooth_coeff, void* stream);
-
 /* Multi-hand tracking of one stream between parse and MANO: a stable track id per detected hand and one OneEuro
- * bank per track, for up to K hands per side (the parse's max_hands_per_side).  The B images of a call are B
+ * bank per track, for up to K hands per side (the parse's max_hands_per_side).  The filter replaces OneEuroFilter /
+ * LowPassFilter (acr/utils.py:1485-1527), smooth_results (:1478-1482), smooth_global_rot_matrix (:1466-1470) and the
+ * per-frame host loop of acr/main.py:69-83 (SURVEY.md 8f-3): K = 1 with the gate open (>= 90) and no miss limit
+ * (max_missed = 2^31 - 1) is the reference's per-hand-type smoothing, one bank per side.  The B images of a call are B
  * consecutive frames in time order; rows are in the parse's layout (row_src (n,4): image, side, flat centre cell
  * y*64+x, unused).  Per frame and side: live tracks match detections greedily by integer squared cell distance
  * within `gate` cells (ties by slot, then row); a track unmatched for more than `max_missed` consecutive frames
@@ -248,8 +238,8 @@ int acr_b200_one_euro_smooth(float* poses, float* betas, const int32_t* hand_typ
  * Track ids are 2*c + side with a per-side birth counter c, never reused.  tests/track_ref.py is the statement.
  * track_id (n_max) gets each row's id, -1 for a row that is no detection (detection_flag <= 0, at or past *n_dev,
  * out of range, or out of time order -- such rows are left untouched).  With poses (n,48) and betas (n,10), each
- * tracked detection is filtered in place through its track's bank with acr_b200_one_euro_smooth's arithmetic (a
- * track's first frame passes the pose's 45 values and the betas through); with both NULL only ids are computed.
+ * tracked detection is filtered in place through its track's bank with that filter (a track's first frame passes
+ * the pose's 45 values and the betas through); with both NULL only ids are computed.
  * `state`: device buffer of acr_b200_track_state_bytes(K) bytes, zeroed = no tracks.  One launch over B frames
  * equals B launches of one frame, bit for bit.  K outside 1..16, B < 1, n_max outside 0..2*K*B, gate or max_missed
  * < 0, a NULL state / row_src / track_id, exactly one of poses and betas NULL, or smooth_coeff <= 0 with poses is

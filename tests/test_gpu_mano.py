@@ -117,15 +117,16 @@ def test_mano_batch512_mixed_sides_and_edges(wrapper, assets):
     assert rel_err(out["pj2d_org"].cpu().numpy()[:N - 5], ref["pj2d_org"][:N - 5]) < TOL
 
 
-def test_one_euro_smoothing_device():
-    """acr_b200_one_euro_smooth vs the reference's filter objects (smooth_golden.npz), frame by frame."""
+def test_open_gate_tracker_smoothing_golden():
+    """The K = 1 tracker with the gate open and no miss limit (the per-hand-type smoothing of
+    ACR.process_results) vs the reference's filter objects (smooth_golden.npz), frame by frame."""
     from acr_b200 import ops
     g = np.load(os.path.join(GOLDEN, "smooth_golden.npz"))
-    st = ops.OneEuroState("cuda")
-    ht = torch.tensor([0, 1], dtype=torch.int32).cuda()
+    tr = ops.HandTracker("cuda", 1, ops.TRACK_GATE_OPEN, ops.TRACK_NO_MISS_LIMIT, 4.0)
+    rows = torch.tensor([[0, 0, 0, 0], [0, 1, 0, 0]], dtype=torch.int32).cuda()
     for t in range(g["poses"].shape[0]):
         poses = torch.from_numpy(g["poses"][t].copy()).cuda()
         betas = torch.from_numpy(g["betas"][t].copy()).cuda()
-        ops.one_euro_smooth(poses, betas, st, 4.0, hand_type=ht, detection_flag=torch.from_numpy(g["det"][t].copy()).cuda())
+        ops.track_rows(tr, 1, rows, torch.from_numpy(g["det"][t].copy()).cuda(), poses, betas)
         assert np.abs(poses.cpu().numpy() - g["out_poses"][t]).max() < 5e-5, t
         assert np.abs(betas.cpu().numpy() - g["out_betas"][t]).max() < 1e-6, t

@@ -1,6 +1,7 @@
 """The fp32 tail on the GPU (acr_b200_mano_forward with its projection outputs, acr_b200_cam_trans,
-acr_b200_rot6d_to_aa, acr_b200_rodrigues, acr_b200_one_euro_smooth) against the float64 statements of
-tests/tail_ref.py, per element and within their derived bounds, on the kernels' masking, alignment and branch edges.
+acr_b200_rot6d_to_aa, acr_b200_rodrigues, the OneEuro smoothing of acr_b200_track_hands) against the float64
+statements of tests/tail_ref.py, per element and within their derived bounds, on the kernels' masking, alignment and
+branch edges.
 
 Every call goes through the C ABI with caller-owned buffers: an output is a 16-byte aligned window inside a larger
 buffer, the window prefilled with one NaN pattern and the guards around it with another, so that after a launch the
@@ -416,21 +417,34 @@ def smooth_sequence(frames, seed):
 
 
 class SmoothRig:
-    """poses (2,48), betas (2,10) and the state, each a guarded window the kernel updates in place."""
+    """poses (2,48), betas (2,10) and the state of the K = 1 tracker with the gate open and no miss limit (the
+    per-hand-type smoothing: one track and bank per side), each a guarded window the kernel updates in place."""
 
-    def __init__(self, rows=2):
-        self.nstate = int(L.load().acr_b200_one_euro_state_floats())
-        self.p, self.b, self.s = Win(rows, 48), Win(rows, 10), Win(self.nstate)
-        self.s.buf[NG:NG + self.nstate] = 0
+    def __init__(self):
+        from acr_b200 import ops
+        self.gate, self.max_missed = ops.TRACK_GATE_OPEN, ops.TRACK_NO_MISS_LIMIT
+        nstate = int(L.load().acr_b200_track_state_bytes(1)) // 4
+        self.side = nstate // 2                 # int32 words per side: births, slot record, bank
+        self.p, self.b, self.s = Win(2, 48), Win(2, 10), Win(nstate)
+        self.s.buf[NG:NG + nstate] = 0
+        self.ids = torch.zeros(2, dtype=torch.int32, device="cuda")
+
+    def bank(self, s, h):
+        """Side h's filter bank in a state snapshot: the side's words from byte 16 + 16 K on."""
+        return s[h * self.side + (16 + 16) // 4:(h + 1) * self.side]
 
     def load(self, poses, betas):
         self.p.buf[NG:NG + self.p.numel] = dev(poses).view(torch.int32).flatten()
         self.b.buf[NG:NG + self.b.numel] = dev(betas).view(torch.int32).flatten()
 
-    def run(self, coeff, hand_type=None, det=None, n_dev=None, rows=2):
-        keep = [dev(hand_type, np.int32), dev(det), None if n_dev is None else dev([n_dev], np.int32)]
-        rc = L.load().acr_b200_one_euro_smooth(self.p.ptr, self.b.ptr, L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2]), rows,
-                                               self.s.ptr, float(coeff), stream())
+    def run(self, coeff, hand_type=(0, 1), det=None, n_dev=None):
+        """One frame: row r is a hand of side hand_type[r] (any cell: the gate is open)."""
+        rows = np.zeros((2, 4), np.int32)
+        rows[:, 1] = hand_type
+        keep = [dev(rows, np.int32), dev(det), None if n_dev is None else dev([n_dev], np.int32)]
+        rc = L.load().acr_b200_track_hands(self.p.ptr, self.b.ptr, L.ptr(keep[0]), L.ptr(keep[1]), L.ptr(keep[2]), 2,
+                                           1, 1, self.gate, self.max_missed, float(coeff), self.s.ptr,
+                                           L.ptr(self.ids), stream())
         torch.cuda.synchronize()
         return rc
 
@@ -439,12 +453,11 @@ class SmoothRig:
 
 
 @pytest.mark.parametrize("coeff", [0.5, 4.0, 30.0])
-def test_one_euro_every_frame(coeff):
+def test_open_gate_tracker_one_euro_every_frame(coeff):
     st = Stats()
     frames = 300
     poses, betas, det = smooth_sequence(frames, 800)
     rig, banks, seen = SmoothRig(), [T.OneEuro64(coeff), T.OneEuro64(coeff)], [False, False]
-    bank = rig.nstate // 2
     ht = np.array([0, 1])
     for t in range(frames):
         rig.load(poses[t], betas[t])
@@ -455,7 +468,7 @@ def test_one_euro_every_frame(coeff):
             pin, bin_ = poses[t, h].view(np.int32), betas[t, h].view(np.int32)
             if not det[t, h] > 0:      # an undetected hand: its row and its bank are untouched
                 assert (p[h].view(np.int32) == pin).all() and (b[h].view(np.int32) == bin_).all()
-                assert (s1[h * bank:(h + 1) * bank] == s0[h * bank:(h + 1) * bank]).all()
+                assert (rig.bank(s1, h) == rig.bank(s0, h)).all()
                 continue
             r = banks[h].process(poses[t, h], betas[t, h])
             if not seen[h]:            # a first frame passes pose and betas through bit for bit
@@ -468,53 +481,33 @@ def test_one_euro_every_frame(coeff):
             st.within("root (as a rotation)", np.array([e]), np.zeros(1),
                       np.array([T.smoothed_root_bound(r["b_M"], r["qnorm"])]))
     assert all(seen)
-    st.show(f"one_euro_smooth smooth_coeff={coeff}, {frames} frames")
+    st.show(f"one_euro smoothing smooth_coeff={coeff}, {frames} frames")
 
 
-def test_one_euro_banks_masks_and_reset():
+def test_open_gate_tracker_one_euro_masks_and_reset():
     poses, betas, _ = smooth_sequence(12, 801)
-    a, b = SmoothRig(), SmoothRig()
-    for t in range(6):     # hand_type NULL: bank = row, the same as hand_type [0, 1]
-        for rig, ht in ((a, None), (b, np.array([0, 1]))):
-            rig.load(poses[t], betas[t])
-            assert rig.run(4.0, ht) == L.OK
-        for x, y in zip(a.get(), b.get()):
-            assert (x.view(np.int32) == y.view(np.int32)).all()
+    a = SmoothRig()
+    for t in range(6):
+        a.load(poses[t], betas[t])
+        assert a.run(4.0) == L.OK
     # n_dev = 1 filters row 0 only
     a.load(poses[6], betas[6])
     _, _, s0 = a.get()
-    assert a.run(4.0, None, None, n_dev=1) == L.OK
+    assert a.run(4.0, n_dev=1) == L.OK
     p, bb, s1 = a.get()
-    half = a.nstate // 2
     assert (p[1].view(np.int32) == poses[6, 1].view(np.int32)).all() and (bb[1].view(np.int32) == betas[6, 1].view(np.int32)).all()
-    assert (s1[half:] == s0[half:]).all() and (s1[:half] != s0[:half]).any()
+    assert (a.bank(s1, 1) == a.bank(s0, 1)).all() and (a.bank(s1, 0) != a.bank(s0, 0)).any()
     assert (p[0, 3:] != poses[6, 0, 3:]).any()
-    # a zeroed state (OneEuroState.reset) makes the next frame a first frame
+    # a reset tracker (HandTracker.reset) makes the next frame a first frame
     from acr_b200 import ops
-    state = ops.OneEuroState("cuda")
+    tracker = ops.HandTracker("cuda", 1, ops.TRACK_GATE_OPEN, ops.TRACK_NO_MISS_LIMIT, 4.0)
+    rows = dev([[0, 0, 0, 0], [0, 1, 0, 0]], np.int32)
     for t in range(3):
         pt, bt = dev(poses[t]), dev(betas[t])
-        ops.one_euro_smooth(pt, bt, state, 4.0)
+        ops.track_rows(tracker, 1, rows, None, pt, bt)
     assert (pt[:, 3:].cpu().numpy() != poses[2][:, 3:]).any()
-    state.reset()
+    tracker.reset()
     pt, bt = dev(poses[3]), dev(betas[3])
-    ops.one_euro_smooth(pt, bt, state, 4.0)
+    ops.track_rows(tracker, 1, rows, None, pt, bt)
     assert (pt[:, 3:].cpu().numpy().view(np.int32) == poses[3][:, 3:].view(np.int32)).all()
     assert (bt.cpu().numpy().view(np.int32) == betas[3].view(np.int32)).all()
-
-
-def test_one_euro_rejects_more_rows_than_banks():
-    """The state has one bank per hand type: n_max > 2 is an argument error before any launch.  Every buffer here
-    holds three rows and hand_type names existing banks only, so the call stays inside its buffers in any case."""
-    from acr_b200 import ops
-    rig = SmoothRig(rows=3)
-    rng = np.random.default_rng(9)
-    poses, betas = rng.standard_normal((3, 48)).astype(np.float32), rng.standard_normal((3, 10)).astype(np.float32)
-    rig.load(poses, betas)
-    before = rig.get()
-    assert rig.run(4.0, np.array([0, 1, 0]), rows=3) == -1          # ACR_B200_EINVAL
-    assert b"one_euro_smooth" in L.load().acr_b200_last_error()
-    for x, y in zip(before, rig.get()):
-        assert (x.view(np.int32) == y.view(np.int32)).all()
-    with pytest.raises(L.AcrB200Error):
-        ops.one_euro_smooth(dev(poses), dev(betas), ops.OneEuroState("cuda"), 4.0, hand_type=dev([0, 1, 0], np.int32))

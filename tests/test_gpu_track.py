@@ -1,7 +1,7 @@
 """GPU: multi-hand tracking (acr_b200_track_hands, acr_b200.ops.HandTracker) against the statement of
 tests/track_ref.py: ids exactly, smoothed values within tests/tail_ref.OneEuro64's per-element bounds (one bank per
-track), untouched rows bit for bit; at K = 1 with the gates open it is acr_b200_one_euro_smooth bit for bit.  Then
-the pipeline at K = 4 on the multi-hand synthetic network: fused_forward, CUDA-graph replay and the eager path."""
+track), untouched rows bit for bit.  Then the pipeline at K = 4 on the multi-hand synthetic network: fused_forward,
+CUDA-graph replay and the eager path."""
 import numpy as np
 import pytest
 import torch
@@ -10,7 +10,6 @@ from acr_b200 import lib as L
 from tests import tail_ref as T
 from tests.test_cpu_track import random_scene
 from tests.test_gpu_parse_topk import _frames, hands_per_side, multi  # noqa: F401  (the module's fixture)
-from tests.test_gpu_tail import SmoothRig, smooth_sequence
 from tests.track_ref import GATE_OPEN, NO_MISS_LIMIT, Tracker, parse_rows
 
 pytestmark = pytest.mark.gpu
@@ -136,24 +135,6 @@ def test_rows_past_n_dev_and_malformed_rows_are_untouched():
 
 
 # -------------------------------------------------------------------------------------------- bit-for-bit anchors
-@pytest.mark.parametrize("coeff", [0.5, 4.0, 30.0])
-def test_k1_open_gates_is_one_euro_smooth(coeff):
-    frames = 300
-    poses, betas, det = smooth_sequence(frames, 800)
-    old, rig = SmoothRig(), Rig(1)
-    rows = np.array([[0, 0, 0, -1], [0, 1, 0, -1]], np.int32)
-    for t in range(frames):
-        old.load(poses[t], betas[t])
-        assert old.run(coeff, np.array([0, 1]), det[t]) == L.OK
-        po, bo, _ = old.get()
-        rc, ids, p, b = rig.run(rows, det[t], 1, poses[t], betas[t], gate=GATE_OPEN, max_missed=NO_MISS_LIMIT,
-                                coeff=coeff)
-        assert rc == L.OK
-        assert (p.view(np.int32) == po.view(np.int32)).all(), t
-        assert (b.view(np.int32) == bo.view(np.int32)).all(), t
-        assert ids.tolist() == [h if det[t, h] > 0 else -1 for h in range(2)]
-
-
 @pytest.mark.parametrize("K", [2, 16])
 def test_one_launch_equals_single_frames_and_repeats(K):
     B = 40

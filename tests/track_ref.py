@@ -5,7 +5,7 @@ Rows come in the parse's layout and order: ``row_src`` (n,4) = image, side, flat
 centre map, and a fourth column the tracker does not read; side-major, then image-major, then by rank (descending
 score).  Each side is tracked on its own, in K slots.  A live slot holds its id, the cell of its last matched
 detection, its count of consecutive missed frames and a 64-element OneEuro bank (45 pose values, 10 betas, 9 root-
-matrix entries, as acr_b200_one_euro_smooth's).
+matrix entries: the quantities of the reference's smooth_results).
 
 Which rows are detections.  Walking the rows [0, min(n_dev, n_max)) of one side in table order, a row is skipped
 (track id -1, left untouched) when its image is outside [0, B), its cell outside [0, 4096), or its image below that of
@@ -24,11 +24,11 @@ Per frame b = 0..B-1 and side s, in this order:
 A frame with no detection of a side still runs steps 2 (every live slot misses).  gate >= 90 never rejects a pair
 (63^2 + 63^2 < 90^2).
 
-Filtering: each detection with a track goes through its track's bank with acr_b200_one_euro_smooth's arithmetic
-(te = 1/30 whatever the gap).  A newborn track's first frame passes the pose's 45 values and the betas through; the
-root, as every frame's, is the filtered matrix taken back to an axis angle (for a first frame the Rodrigues round
-trip of the input, exactly as acr_b200_one_euro_smooth's first frame).  Frames without a detection leave the bank
-untouched.  A zeroed state is no tracks and both counters at zero.
+Filtering: each detection with a track goes through its track's bank with the reference's OneEuroFilter
+(acr/utils.py:1485-1527, te = 1/30 whatever the gap).  A newborn track's first frame passes the pose's 45 values and
+the betas through; the root, as every frame's, is the filtered matrix taken back to an axis angle (for a first frame
+the Rodrigues round trip of the input, as the reference's filter returns a first frame unchanged).  Frames without a
+detection leave the bank untouched.  A zeroed state is no tracks and both counters at zero.
 """
 import numpy as np
 
