@@ -317,6 +317,83 @@ class ACR(nn.Module):
         return replay
 
     @torch.no_grad()
+    def capture_jpeg_graph(self, batch: int, max_coded_bytes: int, max_frame_bytes: int, tracker=None, device=None,
+                           max_blocks: int = None):
+        """``capture_frames_graph`` from JPEG files: one CUDA graph of the device JPEG decode (acr_b200.jpeg), the
+        ragged pre-processing and ``fused_forward``.  Returns ``replay(encoded_list) -> (bufs, mano)`` for exactly
+        ``batch`` baseline JPEG files (bytes-like) whose entropy-coded bytes sum to at most ``max_coded_bytes`` and
+        whose decoded H*W*3 bytes sum to at most ``max_frame_bytes``; ``max_blocks`` caps the 8x8 coefficient blocks
+        (default ``max_frame_bytes // 48 + 64 * batch``: enough for every sampling when each frame is at least 18
+        pixels on each side; thin frames pad more per pixel, a 1x1920 frame needs 720 blocks, so give a larger cap).
+        The replay parses the headers and checks the caps and the supported features before anything is enqueued
+        (ValueError / acr_b200.jpeg.JpegUnsupported); the decode's grids are sized by the caps and the device skips
+        work past each file's size.  Corrupt entropy-coded data sets the per-file status words and gives that frame
+        an all-black image; ``replay.jpeg.raise_on_status()`` waits and raises.  Like ``capture_graph``, the graph
+        is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with a multi-stream tracker the replay is
+        ``replay(encoded_list, stream_ids, stream_begin=None)``."""
+        from acr.result_parser import ResultParser
+        from acr_b200 import jpeg
+        from acr_b200.preprocess import RaggedFrames
+        import cv2
+        import numpy as np
+        K = ResultParser.hands_per_side()
+        _check_tracker(tracker, K)
+        dev = torch.device(device) if device is not None else next(self.model.parameters()).device
+        if max_blocks is None:
+            max_blocks = max_frame_bytes // 48 + 64 * batch
+        rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
+        jb = jpeg.JpegBatch(batch, max_coded_bytes, max_frame_bytes, -(-max_coded_bytes // jpeg.CHUNK) + batch,
+                            max_blocks, dev, out=rf.packed)
+        warm = [cv2.imencode(".jpg", np.full((1, 1, 3), 255, np.uint8))[1].tobytes()] * batch
+
+        def load(encoded, lay):
+            shapes = [(int(d["H"]), int(d["W"])) for d in lay.desc]
+            rf.load_shapes(shapes)
+            jb.load(encoded, lay)
+
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
+            load(warm, jb.prepare(warm, exact=True)[0])
+            for _ in range(2):
+                jb.launch(batch)
+                self.fused_forward(*rf.launch())
+        cur.wait_stream(side)
+        torch.cuda.synchronize(dev)
+        streams = _stream_buffers(tracker, batch, dev)
+        if tracker is not None:
+            tracker.ids(batch)
+            if streams is not None:
+                tracker.workspace(batch)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            jb.launch(batch)
+            bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker, stream_ids=streams and streams[0],
+                                            stream_begin=streams and streams[1])
+
+        def replay_one(encoded_list):
+            _check_hands_per_side(K)
+            encoded_list = list(encoded_list)
+            load(encoded_list, jb.prepare(encoded_list, exact=True)[0])
+            graph.replay()
+            return bufs, mano
+
+        def replay_streams(encoded_list, stream_ids=None, stream_begin=None):
+            _check_hands_per_side(K)
+            encoded_list = list(encoded_list)
+            lay, _ = jb.prepare(encoded_list, exact=True)   # every check before the stream ids are copied
+            _load_streams(streams, stream_ids, stream_begin)
+            load(encoded_list, lay)
+            graph.replay()
+            return bufs, mano
+
+        replay = replay_one if streams is None else replay_streams
+        replay.graph, replay.frames, replay.jpeg, replay.hands_per_side = graph, rf, jb, K
+        replay.static_streams = streams
+        return replay
+
+    @torch.no_grad()
     def single_image_forward(self, image_rgb_u8_512, path=None):
         meta = {'image': image_rgb_u8_512[None] if image_rgb_u8_512.dim() == 3 else image_rgb_u8_512,
                 'offsets': torch.tensor([[512., 512, 0, 0, 0, 0, 0, 0, 0, 0]]), 'batch_ids': torch.arange(1)}

@@ -144,3 +144,11 @@ def img_preprocess(image, imgpath=None, input_size=512, single_img_input=False, 
     if imgpath is not None:
         input_data.update({'imgpath': imgpath, 'name': os.path.basename(imgpath)})
     return input_data
+
+
+def img_preprocess_jpeg(encoded_list, paths=None, input_size=512, host_fallback=False):
+    """``img_preprocess`` of a list of JPEG files (encoded bytes): decoded on the device (acr_b200.jpeg.decode, equal
+    to cv2.imdecode), then padded and resized in one launch.  Returns the same dict as ``img_preprocess`` of the
+    decoded frames.  Unsupported files raise before anything is enqueued unless ``host_fallback``."""
+    from acr_b200 import jpeg
+    return img_preprocess(jpeg.decode(encoded_list, host_fallback=host_fallback), paths, input_size)

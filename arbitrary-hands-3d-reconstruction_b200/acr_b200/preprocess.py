@@ -115,6 +115,19 @@ def _frame_hw(i: int, f) -> Tuple[int, int]:
     return int(f.shape[0]), int(f.shape[1])
 
 
+def shapes_layout(shapes) -> Tuple[np.ndarray, np.ndarray, int]:
+    """``ragged_layout`` of frames given by their (H, W) only."""
+    desc = np.zeros(len(shapes), FRAME_DTYPE)
+    offsets = np.zeros((len(shapes), 10), np.float32)
+    pos = 0
+    for i, (H, W) in enumerate(shapes):
+        t, r, b, l = paddings_to_square(H, W)
+        desc[i] = (pos, H, W, max(H, W), t, l, 0)
+        offsets[i] = offsets_vector(H, W)
+        pos += H * W * 3
+    return desc, offsets, pos
+
+
 def ragged_layout(frames) -> Tuple[np.ndarray, np.ndarray, int]:
     """Layout of a list of (H_i, W_i, 3) uint8 frames packed back to back -> (descriptors (n,) FRAME_DTYPE,
     offsets vectors (n,10) float32, packed bytes).  Frame i starts at the sum of H_j * W_j * 3 over j < i.  Raises
@@ -217,6 +230,30 @@ class RaggedFrames:
             self._copied.record()
             if not host:
                 torch.cat([f.reshape(-1) for f in frames], out=self.packed[:total])
+        self.n = n
+        return n
+
+    def load_shapes(self, shapes) -> int:
+        """Like ``load`` for frames that are already packed in ``self.packed`` (written there by the device, e.g. by
+        the JPEG decoder): copies only the descriptors of frames of the given (H, W), on the current stream."""
+        if len(shapes) == 0:
+            raise ValueError("a ragged batch needs at least one frame")
+        desc, _, total = shapes_layout(shapes)
+        n = len(shapes)
+        if self.exact and n != self.max_frames:
+            raise ValueError(f"this ragged batch takes exactly {self.max_frames} frames, got {n}")
+        if n > self.max_frames or total > self.max_bytes:
+            raise ValueError(f"{n} frames of {total} bytes exceed the capacity of {self.max_frames} frames / "
+                             f"{self.max_bytes} bytes")
+        stage = self._staging(self.meta_bytes)
+        np_stage = stage.numpy()
+        np_stage[:n * FRAME_DTYPE.itemsize] = desc.view(np.uint8)
+        d0 = self.desc.numel()
+        np_stage[d0:d0 + 4 * n] = desc["side"].astype(np.int32).view(np.uint8)
+        with torch.cuda.device(self.device):
+            self.buf[:self.meta_bytes].copy_(stage[:self.meta_bytes], non_blocking=True)
+            self._copied = torch.cuda.Event()
+            self._copied.record()
         self.n = n
         return n
 

@@ -497,6 +497,71 @@ int acr_b200_pack_conv(const float* w_oihw, const float* conv_bias, const float*
                        int cout, int cin, int k, int cout_pad, int cin_pad, int act_dtype,
                        void* w_packed_host, float* bias_host);
 
+/* ---- baseline JPEG decoding (csrc/jpeg.cu) ------------------------------------------------------------------
+ * Replaces the host decode of every input mode of the reference (cv2.imread in image / folder mode, and the
+ * read-back of the frames split_frame writes in video mode; /root/reference/demo.py, acr/utils.py).  The host parses
+ * the headers (acr_b200/jpeg.py) into one acr_b200_jpeg_frame per file; the entropy-coded segments travel
+ * untouched, packed back to back.  Output: BGR HWC frames packed back to back, equal to cv2.imdecode(buf,
+ * IMREAD_COLOR) (libjpeg-turbo: JDCT_ISLOW, fancy upsampling) byte for byte.                                      */
+#define ACR_B200_JPEG_CHUNK 256  /* entropy-coded bytes per decoder thread */
+#define ACR_B200_JPEG_MAX_SCAN_BYTES (1 << 28)  /* coded_len must be below this: positions are int32 bit offsets */
+
+/* A Huffman table in lookup form.  1424 bytes. */
+typedef struct acr_b200_jpeg_huff {
+  uint16_t lut[512];   /* next 9 bits -> (code length << 8) | symbol; 0 when the code is longer than 9 bits */
+  int32_t maxcode[18]; /* largest code of each length 1..16, -1 if none; [17] = INT32_MAX */
+  int32_t valoff[18];  /* symbol of code c of length l = huffval[c + valoff[l]] */
+  uint8_t huffval[256];
+} acr_b200_jpeg_huff;
+
+/* One file of a batch.  Component c's plane is comp_bw[c] x comp_bh[c] blocks (whole MCUs); its blocks start at
+ * block coef_offset + comp_block0[c] of the workspace.  Block k of an MCU belongs to component slot_comp[k], at
+ * (slot_dy[k], slot_dx[k]) inside the MCU.  chunk_begin / block_begin: the frame's first chunk (of
+ * ACR_B200_JPEG_CHUNK coded bytes) and block in the batch's numbering.  9112 bytes. */
+typedef struct acr_b200_jpeg_frame {
+  int64_t coded_offset; /* entropy-coded segment: bytes [coded_offset, coded_offset + coded_len) of `coded` */
+  int64_t out_offset;   /* first BGR byte of the frame in `out_bgr` */
+  int64_t coef_offset;  /* = block_begin */
+  int32_t coded_len, H, W, ncomp;
+  int32_t mcus_x, mcus_y, bpm, restart; /* blocks per MCU; restart interval in MCUs, 0 = none */
+  int32_t chunk_begin, n_chunks, block_begin, n_blocks;
+  int32_t comp_h[3], comp_v[3];   /* sampling factors (grey: 1, 1) */
+  int32_t comp_bw[3], comp_bh[3]; /* plane size in blocks */
+  int32_t comp_w[3], comp_hgt[3]; /* component size in samples (libjpeg's downsampled_width / _height) */
+  int32_t comp_block0[3];
+  int32_t reserved;
+  int8_t slot_comp[8], slot_dy[8], slot_dx[8];
+  uint16_t quant[3][64]; /* natural order */
+  acr_b200_jpeg_huff dc[3], ac[3];
+} acr_b200_jpeg_frame;
+
+/* Status bits of acr_b200_jpeg_decode, per frame (0 = decoded). */
+#define ACR_B200_JPEG_BAD_CODE 1     /* a code that is not in the table, or an AC run past the block */
+#define ACR_B200_JPEG_TRUNCATED 2    /* the segment ends before the last MCU */
+#define ACR_B200_JPEG_BAD_RESTART 4  /* a restart marker out of place or out of sequence */
+#define ACR_B200_JPEG_BAD_MARKER 8   /* another marker inside the entropy-coded data */
+#define ACR_B200_JPEG_BAD_LENGTH 16  /* more coded blocks than the frame has */
+
+/* Workspace of acr_b200_jpeg_decode for at most max_chunks chunks and max_blocks blocks over the batch. */
+size_t acr_b200_jpeg_workspace_bytes(int64_t max_chunks, int64_t max_blocks);
+/* Byte offset in that workspace of the coefficient blocks, which stay valid after a decode: block k of the batch
+ * (frame.coef_offset + comp_block0[c] + row * comp_bw[c] + column) is 64 int16 quantised coefficients in natural
+ * order, DC included.  Frames with status != 0 have undefined coefficients. */
+size_t acr_b200_jpeg_coef_offset(int64_t max_chunks);
+
+/* Decode n frames (frames: device descriptors) from `coded` (coded_bytes bytes) into `out_bgr` (out_bytes bytes),
+ * in a fixed number of launches: speculative Huffman decoding (one thread per chunk, started at a guessed code
+ * boundary), one CTA per frame to synchronise the chunks and prefix their block counts and DC predictions, the
+ * coefficient stores, the islow IDCT, and fancy upsampling with colour conversion.  Grids are sized by max_chunks,
+ * max_blocks and out_bytes; the device skips work past the batch's real totals, so a CUDA graph can replay it with
+ * other files.  status (device, n int32) gets each frame's ACR_B200_JPEG_* bits; a frame with status != 0 gets an
+ * all-black image (none when its descriptor does not fit the buffers, status bit 256).  Every read stays inside the
+ * frame's segment, and every store inside its own output.
+ * Frames whose descriptor has ncomp == 0 are skipped (left untouched in out_bgr, status 0).                      */
+int acr_b200_jpeg_decode(const uint8_t* coded, int64_t coded_bytes, const acr_b200_jpeg_frame* frames, int n,
+                         int64_t max_chunks, int64_t max_blocks, void* workspace, size_t workspace_bytes,
+                         uint8_t* out_bgr, int64_t out_bytes, int32_t* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
