@@ -318,7 +318,7 @@ int conv_bottleneck_prepare(const ConvArgs& a1, const ConvArgs& a2, const ConvAr
   pl->cchunks = a1.cin_pad / 64;
   p.res_stride = a3.res.pix_stride; p.out_stride = a3.out.pix_stride;
   p.H = H; p.W = W;
-  p.tiles_x = W / TILE_X; p.tiles_per_img = p.tiles_x * (H / TILE_Y);
+  p.tiles_x = W / TILE_X; p.tiles_per_img = p.tiles_x * (H / BNK_TILE_Y);   // 16 x 8 tiles
   p.total_tiles = p.tiles_per_img * a1.batch;
   pl->grid = p.total_tiles < num_sms() ? p.total_tiles : num_sms();
   *out = pl;

@@ -63,7 +63,7 @@ def conv_classes(recs, batch, blocks=(), bottlenecks=()):
     flat rows per 16x16 tile, 2x its pixels; the x-paired form issues its side taps at full width, 4/3).
     `bottlenecks`: first records of the Bottlenecks that run as one fused launch (csrc/conv_bottleneck.cuh), a class of
     their own (k "1+3+1", cin = the block input's channels): FLOP of the three convs, bytes in + residual (when it is not
-    the input) + out, and the issued FLOP (conv1 runs 8 M blocks of 64 flat rows per 16x16 tile, 2x its pixels)."""
+    the input) + out, and the issued FLOP (conv1 runs 4 M blocks of 64 flat rows per 16x8 tile, 2x its pixels)."""
     agg = collections.OrderedDict()
     blocks, bottlenecks = set(blocks), set(bottlenecks)
     for i, r in enumerate(recs):
