@@ -405,6 +405,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
   const uint32_t b_block16 = P.b_block_bytes >> 4, a_stage16 = P.a_stage_bytes >> 4;
   const int cchunks = P.cchunks, taps = P.taps, nsub = P.nsub;
   const bool tma_out = P.tma_out != 0;   // (16-bit outputs only: conv_tc_prepare)
+  const bool plain = !tma_out && !P.has_res && !P.pow11_ch0 && P.n_ext == 0;   // short epilogue (see below)
   const int wg_thread = threadIdx.x & 127;
   const uint32_t stage_wg = stage_base + (uint32_t)wg * 8192u;      // this warpgroup's output slab (TMA-store epilogue)
   const uint32_t is_lane0 = lane == 0 ? 1u : 0u;
@@ -603,6 +604,40 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_con
     const int oy0 = (rem / P.tiles_x) * TILE_Y + rg * 8 + 2 * wq, ox = (rem % P.tiles_x) * TILE_X + h * HALF_X + (lane >> 2);
     const int cq = 2 * (lane & 3);
     const int ty0 = (rem / P.tiles_x) * TILE_Y + rg * 8, tx0 = (rem % P.tiles_x) * TILE_X + h * HALF_X;   // slab origin
+    if constexpr (!IsF32<T>::value) {
+      if (plain) {
+        // Plain layers (stores from the fragment, no residual, no cam-scale channel, no extra terms): one short
+        // straight-line body per channel pair.  The general loop below carries every optional term; inlined for all
+        // 32 channel pairs of a thread, it is most of the kernel's code, far more than the instruction cache holds,
+        // and it ran several times slower than this loop (DESIGN.md, Conv).  The float operations are those of the
+        // general loop, in the same order.  Columns [0, cols) of the virtual tile are stored: inside it (nsub) and
+        // below cout_pad (npad and n_off are multiples of 16, so the bound holds for a whole group of 8 channels).
+        const int cols = min(nsub, P.npad - n_off);
+        const float* pbias = P.bias_per_image ? P.bias + (size_t)n * P.npad + n_off : s_bias + n_off;
+#pragma unroll
+        for (int g = 0; g < NT / 64; ++g) {
+          if (64 * g >= cols) break;
+#pragma unroll
+          for (int r2 = 0; r2 < 2; ++r2) {
+            const int oy = oy0 + r2;
+            const size_t pix = DECONV ? ((size_t)n * P.Ho + 2 * oy + (par >> 1)) * P.Wo + 2 * ox + (par & 1)
+                                      : ((size_t)n * P.Ho + oy) * P.Wo + ox;
+            const size_t o = pix * P.out_stride + n_off + cq;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * g + jj;
+              if (8 * j >= cols) break;
+              const float2 b = *reinterpret_cast<const float2*>(pbias + 8 * j + cq);
+              float f0 = acc[4 * j + 2 * r2] + b.x, f1 = acc[4 * j + 2 * r2 + 1] + b.y;
+              if (P.relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+              if (P.out_f32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(P.out) + o + 8 * j) = make_float2(f0, f1);
+              else *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(P.out) + o + 8 * j) = pack2<T>(f0, f1);
+            }
+          }
+        }
+        continue;
+      }
+    }
     // bias: per CTA from shared memory, or (folded part-head conv) one row per image from global
     const float* bsrc = P.bias_per_image ? P.bias + (size_t)n * P.npad + n_off : s_bias + n_off;
     // the channels come in groups of 64: with the TMA-store epilogue one group of the warpgroup's 64 pixels is one
