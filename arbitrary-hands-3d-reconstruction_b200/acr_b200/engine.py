@@ -153,8 +153,7 @@ class Engine:
         from .netspec import WIDTHS
         # Folding the coarse fuse sums into the producing conv (ACR_B200_FOLD_FUSE=1) is an opt-in: it trades the fuse
         # kernels for extra latency-bound loads in the conv epilogue.  Tensor-core plans only.
-        self.spec: NetSpec = build_acr_spec(input_size, merge_stems=os.environ.get("ACR_B200_MERGE_STEMS", "1") != "0",
-                                            widths=tuple(widths) if widths else WIDTHS,
+        self.spec: NetSpec = build_acr_spec(input_size, widths=tuple(widths) if widths else WIDTHS,
                                             fold_fuse=(os.environ.get("ACR_B200_FOLD_FUSE", "0") != "0"
                                                        and act_dtype != torch.float32 and not debug_ref_conv),
                                             backbone=backbone)
@@ -475,8 +474,7 @@ class Engine:
             if self.f32 or r["kind"] != L.OP_CONV or a.get("k") != 3 or a.get("s") != 2 or a.get("merged") or "stem" in a:
                 return False
             x, y = r["ins"][0], r["out"]
-            return (x.C == 32 and x.base is None and x.dtype == "act" and x.W % 32 == 0 and y.H % 16 == 0 and y.W % 16 == 0
-                    and os.environ.get("ACR_B200_S2X", "1") != "0")
+            return x.C == 32 and x.base is None and x.dtype == "act" and x.W % 32 == 0 and y.H % 16 == 0 and y.W % 16 == 0
 
         # ---- weights + C op records
         f32 = lambda k: np.ascontiguousarray(sd[k], np.float32)
@@ -503,7 +501,7 @@ class Engine:
                 o.cin_pad = _rup(x.C, 64) if x.C > 32 else _rup(x.C, 16)
                 o.cout_pad = _rup(r["out"].C, 16)
                 if a.get("extra"):
-                    o.shift[0] |= 16    # ACR_CONV_EXTRA: in_[1..] are further terms, nearest-upsampled by 2**shift[j]
+                    o.shift[0] |= L.CONV_EXTRA
                     for q, (_, sh) in enumerate(a["extra"]):
                         o.shift[1 + q] = sh
                 if a.get("deconv"):
@@ -516,22 +514,22 @@ class Engine:
                 elif "fold_side" in a:
                     o.cin_pad = 128
                     o.w_offset[0] = self._pack_raw(blob, self.fold_weights(sd, a["fold_side"]), o.cin_pad, o.cout_pad)
-                    o.shift[0] |= 1     # ACR_CONV_BIAS_PER_IMAGE (aux[0] = bias_img from the part head)
+                    o.shift[0] |= L.CONV_BIAS_PER_IMAGE   # aux[0] = bias_img from the part head
                 elif s2x:
                     o.cin_pad = 64
                     o.w_offset[0], o.w_offset[1] = self._pack_conv(sd, blob, a["w"], a["bn"], a["bias"], 64, o.cout_pad, s2x=True)
-                    o.shift[0] |= 8     # ACR_CONV_S2X
+                    o.shift[0] |= L.CONV_S2X
                 elif pair:
                     o.cin_pad = o.cout_pad = 64
                     o.w_offset[0], o.w_offset[1] = self._pack_conv(sd, blob, a["w"], a["bn"], a["bias"], 64, 64, pair=True)
-                    o.shift[0] |= 4     # ACR_CONV_XPAIR: side taps are 32x32 corners of the 64x64 block
+                    o.shift[0] |= L.CONV_XPAIR
                 elif a.get("merged"):
                     o.w_offset[0], o.w_offset[1] = self._pack_merged(sd, blob, a["w"], a["bn"], a["bias"], a["k"], o.cin_pad,
                                                                      a["merged"])
                 else:
                     o.w_offset[0], o.w_offset[1] = self._pack_conv(sd, blob, a["w"], a["bn"], a["bias"], o.cin_pad, o.cout_pad)
                     if a.get("pow11"):
-                        o.shift[0] |= 2  # ACR_CONV_POW11_CH0
+                        o.shift[0] |= L.CONV_POW11_CH0
                 if r.get("block"):
                     o.shift[0] |= L.CONV_BLOCK | (L.CONV_BLOCK_MID if r["block_mid"] else 0)
                 if r.get("bottleneck"):

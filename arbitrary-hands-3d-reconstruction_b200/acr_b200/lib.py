@@ -16,7 +16,13 @@ LIB_PATH = os.environ.get("ACR_B200_LIB") or os.path.join(os.path.dirname(_HERE)
 OK = 0
 OP_STEM, OP_CONV, OP_FUSE, OP_BILINEAR2X, OP_COORD, OP_POOL, OP_PARTHEAD, OP_CONV_REF, OP_FINALCONV, OP_IM2COL_STEM, OP_STEM_TC = range(1, 12)
 OP_MAXPOOL = 12
-CONV_DECONV = 32      # ACR_CONV_DECONV flag bit (shift[0]) of a CONV op
+# ACR_CONV_* flag bits (shift[0]) of a CONV op
+CONV_BIAS_PER_IMAGE = 1  # ACR_CONV_BIAS_PER_IMAGE: the bias is a per-image fp32 tensor, aux[0]
+CONV_POW11_CH0 = 2    # ACR_CONV_POW11_CH0: output channel 0 -> 1.1**x
+CONV_XPAIR = 4        # ACR_CONV_XPAIR: a 32->32 3x3 conv run x-paired as 64->64, side taps 32x32 corners
+CONV_S2X = 8          # ACR_CONV_S2X: 3x3 stride-2 conv of a dense 32-channel tensor read as x-pairs
+CONV_EXTRA = 16       # ACR_CONV_EXTRA: in[1..] are further terms, nearest-upsampled by 2**shift[j]
+CONV_DECONV = 32      # ACR_CONV_DECONV: transposed conv, kernel 4 stride 2 padding 1
 CONV_BLOCK = 64       # ACR_CONV_BLOCK: this conv and the next are one BasicBlock, run as one launch
 CONV_BLOCK_MID = 128  # ACR_CONV_BLOCK_MID: the fused launch also writes the block's intermediate
 CONV_BOTTLENECK = 256  # ACR_CONV_BOTTLENECK: this conv and the next two are one Bottleneck, run as one launch

@@ -7,14 +7,7 @@ template <typename T, bool XPAIR>
 static int launch_block(const ConvBlockPlan* pl, cudaStream_t st) {
   static unsigned long long configured = 0;
   ACR_CHECK_CUDA(ensure_dynamic_smem(conv_block_kernel<T, XPAIR>, (int)BLK_SMEM, &configured));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(pl->grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = BLK_SMEM; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  ACR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_block_kernel<T, XPAIR>, pl->p));
-  return ACR_B200_OK;
+  return launch_pdl(conv_block_kernel<T, XPAIR>, pl->p, pl->grid, BLK_SMEM, st);
 }
 
 int conv_block_launch(const ConvBlockPlan* pl, cudaStream_t st) {

@@ -7,14 +7,7 @@ template <typename T, int CCHUNKS>
 static int launch_bottleneck(const ConvBottleneckPlan* pl, cudaStream_t st) {
   static unsigned long long configured = 0;
   ACR_CHECK_CUDA(ensure_dynamic_smem(conv_bottleneck_kernel<T, CCHUNKS>, (int)BNK_SMEM, &configured));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(pl->grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = BNK_SMEM; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  ACR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_bottleneck_kernel<T, CCHUNKS>, pl->p));
-  return ACR_B200_OK;
+  return launch_pdl(conv_bottleneck_kernel<T, CCHUNKS>, pl->p, pl->grid, BNK_SMEM, st);
 }
 
 int conv_bottleneck_launch(const ConvBottleneckPlan* pl, cudaStream_t st) {

@@ -53,13 +53,6 @@ static bool tma_out_enabled() {
   return e && atoi(e) != 0;
 }
 
-// The single-box A operand (MODE_P1) is on by default; ACR_B200_P1=0 (read at plan creation) selects the three
-// kx-shifted boxes again (A/B timing).
-static bool p1_enabled() {
-  const char* e = getenv("ACR_B200_P1");
-  return !(e && atoi(e) == 0);
-}
-
 int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   ACR_CHECK_ARG(a.out.H % TILE_Y == 0 && a.out.W % TILE_X == 0, "conv_tc: output %dx%d is not a multiple of the 16x16 super-tile", a.out.H, a.out.W);
   ACR_CHECK_ARG(a.in.pix_stride % 8 == 0 && a.cin_pad % 16 == 0 && a.cout_pad % 16 == 0 && a.cout_pad <= 2048 && a.cin_pad <= 2048,
@@ -92,7 +85,7 @@ int conv_tc_prepare(const ConvArgs& a, int act_dtype, ConvTcPlan** out) {
   p.patch_mode = (a.k == 3 && a.stride == 1) ? 1 : 0;
   // x-paired convs keep the three-box form: their single-box instance mixes full-width and corner MMAs on accumulator
   // subsets within a tap row, which ptxas serialises for lack of registers
-  p.patch1 = (p.patch_mode && ck == 64 && !a.xpair && p1_enabled()) ? 1 : 0;
+  p.patch1 = (p.patch_mode && ck == 64 && !a.xpair) ? 1 : 0;
   p.s2x = a.s2x ? 1 : 0;
   p.deconv = a.deconv ? 1 : 0;
   const cuuint32_t box_rows = p.s2x ? TILE_Y + 1 : ((p.patch_mode || p.deconv) ? TILE_Y + 2 : TILE_Y);

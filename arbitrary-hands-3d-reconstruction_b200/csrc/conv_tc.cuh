@@ -719,24 +719,25 @@ struct ConvTcPlan {
   size_t smem;
 };
 
-static bool pdl_enabled() {   // ACR_B200_PDL=0 disables programmatic dependent launch (A/B timing, debugging)
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ACR_B200_PDL"); v = e ? atoi(e) : 1; }
-  return v != 0;
+// One launch of a conv-family kernel (conv_tc_kernel, conv_block_kernel, conv_bottleneck_kernel) with programmatic
+// dependent launch: it may start while the previous kernel on the stream drains (see pdl_wait).
+template <typename Kernel, typename Params>
+static int launch_pdl(Kernel kernel, const Params& p, int grid, size_t smem, cudaStream_t st) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
+  ACR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, p));
+  return ACR_B200_OK;
 }
 
 template <int CK, typename T, int MODE, int NT>
 static int launch_nt(const ConvTcPlan* pl, cudaStream_t st) {
   static unsigned long long configured = 0;
   ACR_CHECK_CUDA(ensure_dynamic_smem(conv_tc_kernel<CK, T, MODE, NT>, SMEM_BUDGET, &configured));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(pl->grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = pl->smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  ACR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, conv_tc_kernel<CK, T, MODE, NT>, pl->p));
-  return ACR_B200_OK;
+  return launch_pdl(conv_tc_kernel<CK, T, MODE, NT>, pl->p, pl->grid, pl->smem, st);
 }
 
 template <int CK, typename T, int MODE>
@@ -766,11 +767,16 @@ static int launch_mode(const ConvTcPlan* pl, cudaStream_t st) {
       return launch_inst<64, T, MODE_PATCH | MODE_RESIDENT | MODE_XPAIR>(pl, st);
     }
   }
-  switch (mode) {
-    case 0: return launch_inst<CK, T, 0>(pl, st);
-    case 1: return launch_inst<CK, T, 1>(pl, st);
-    case 2: return launch_inst<CK, T, 2>(pl, st);
-    default: return launch_inst<CK, T, 3>(pl, st);
+  if constexpr (CK == 64) {   // every 64-channel-chunk 3x3 stride-1 conv is one of the single-box or x-paired forms above
+    if (pl->p.patch_mode) { set_error("conv_tc: no three-box form of a 64-channel-chunk conv"); return ACR_B200_EINVAL; }
+    return pl->p.b_resident ? launch_inst<64, T, MODE_RESIDENT>(pl, st) : launch_inst<64, T, 0>(pl, st);
+  } else {
+    switch (mode) {
+      case 0: return launch_inst<CK, T, 0>(pl, st);
+      case 1: return launch_inst<CK, T, 1>(pl, st);
+      case 2: return launch_inst<CK, T, 2>(pl, st);
+      default: return launch_inst<CK, T, 3>(pl, st);
+    }
   }
 }
 

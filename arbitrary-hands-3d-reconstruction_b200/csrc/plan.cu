@@ -267,40 +267,28 @@ extern "C" int acr_b200_plan_create(const acr_b200_op* ops, int n_ops, int batch
     }
     if (p->fused[i]) continue;
     const bool tc_conv = op.kind == ACR_OP_CONV && act_dtype != ACR_DT_F32;   // (the TF32 plan ignores the fusion flags)
-    if (tc_conv && act_dtype != ACR_DT_TF32 && (op.shift[0] & ACR_CONV_BOTTLENECK) && fuse_blocks_enabled()) {
-      // one launch for the Bottleneck of ops i .. i + 2 (the engine marks only such triples); the later ops' waits must be
-      // ones op i already has
-      bool ok = i + 2 < n_ops;
-      for (int j = i + 1; ok && j <= i + 2; ++j)
+    // a fused group: the Bottleneck of ops i .. i + 2 or the BasicBlock of ops i and i + 1 (the engine marks only such groups)
+    const bool bottleneck = (op.shift[0] & ACR_CONV_BOTTLENECK) != 0;
+    const int group = bottleneck ? 3 : ((op.shift[0] & ACR_CONV_BLOCK) ? 2 : 1);
+    if (tc_conv && act_dtype != ACR_DT_TF32 && group > 1 && fuse_blocks_enabled()) {
+      // one launch for the group; the later ops' waits must be ones op i already has, so nothing they waited for can be missed
+      bool ok = i + group <= n_ops;
+      for (int j = i + 1; ok && j < i + group; ++j)
         ok = p->ops[j].kind == ACR_OP_CONV && p->ops[j].stream_id == op.stream_id &&
              (p->ops[j].wait_mask & ~op.wait_mask & ~(1 << op.stream_id)) == 0;
       if (!ok) {
-        set_error("op %d: ACR_CONV_BOTTLENECK needs the block's other two convs next, on the same stream", i);
+        set_error(bottleneck ? "op %d: ACR_CONV_BOTTLENECK needs the block's other two convs next, on the same stream"
+                             : "op %d: ACR_CONV_BLOCK needs the block's second conv next, on the same stream", i);
         rc = ACR_B200_EINVAL;
         break;
       }
-      ConvArgs a1, a2, a3;
-      rc = make_conv_args(op, batch, p->arena, p->weights, nullptr, &a1);
-      if (rc == ACR_B200_OK) rc = make_conv_args(p->ops[i + 1], batch, p->arena, p->weights, nullptr, &a2);
-      if (rc == ACR_B200_OK) rc = make_conv_args(p->ops[i + 2], batch, p->arena, p->weights, nullptr, &a3);
-      if (rc == ACR_B200_OK) rc = conv_bottleneck_prepare(a1, a2, a3, act_dtype, &p->bnk[i]);
-      p->fused[i + 1] = p->fused[i + 2] = 1;
-      continue;
-    }
-    if (tc_conv && act_dtype != ACR_DT_TF32 && (op.shift[0] & ACR_CONV_BLOCK) && fuse_blocks_enabled()) {
-      // one launch for the BasicBlock of ops i and i + 1 (the engine marks only such pairs); op i + 1's waits must be
-      // ones op i already has, so nothing that op i + 1 waited for can be missed
-      if (!(i + 1 < n_ops && p->ops[i + 1].kind == ACR_OP_CONV && p->ops[i + 1].stream_id == op.stream_id &&
-            (p->ops[i + 1].wait_mask & ~op.wait_mask & ~(1 << op.stream_id)) == 0)) {
-        set_error("op %d: ACR_CONV_BLOCK needs the block's second conv next, on the same stream", i);
-        rc = ACR_B200_EINVAL;
-        break;
-      }
-      ConvArgs a1, a2;
-      rc = make_conv_args(op, batch, p->arena, p->weights, nullptr, &a1);
-      if (rc == ACR_B200_OK) rc = make_conv_args(p->ops[i + 1], batch, p->arena, p->weights, nullptr, &a2);
-      if (rc == ACR_B200_OK) rc = conv_block_prepare(a1, a2, act_dtype, (op.shift[0] & ACR_CONV_BLOCK_MID) ? 1 : 0, &p->blk[i]);
-      p->fused[i + 1] = 1;
+      ConvArgs a[3];
+      for (int j = 0; j < group && rc == ACR_B200_OK; ++j)
+        rc = make_conv_args(p->ops[i + j], batch, p->arena, p->weights, nullptr, &a[j]);
+      if (rc == ACR_B200_OK)
+        rc = bottleneck ? conv_bottleneck_prepare(a[0], a[1], a[2], act_dtype, &p->bnk[i])
+                        : conv_block_prepare(a[0], a[1], act_dtype, (op.shift[0] & ACR_CONV_BLOCK_MID) ? 1 : 0, &p->blk[i]);
+      for (int j = i + 1; j < i + group; ++j) p->fused[j] = 1;
       continue;
     }
     if (tc_conv) {

@@ -182,7 +182,7 @@ def _sass_by_function():
     return funcs
 
 
-def test_tf32_conv_instances_use_tf32_wgmma_without_spills():
+def test_tf32_conv_instance_set_uses_tf32_wgmma_without_spills():
     if not (os.path.exists(LIB) and os.path.exists(CUOBJDUMP)):
         pytest.skip("library not built or no cuobjdump")
     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -192,15 +192,19 @@ def test_tf32_conv_instances_use_tf32_wgmma_without_spills():
     finally:
         sys.path.pop(0)
     tf = {n: r for n, r in rows.items() if n.startswith("conv_tc_kernel<") and ", float," in n}
-    # CK 64: 4 generic modes + 2 single-box forms; CK 32: 4 generic modes; each at N = 64 and 128
-    assert len(tf) == 20, sorted(tf)
+    # CK 64: the two non-patch modes (1x1 and stride-2 convs) and the two single-box forms (MODE_PATCH | MODE_P1, with
+    # and without MODE_RESIDENT; every tf32 3x3 stride-1 conv with 64-channel chunks takes one); CK 32: the four generic
+    # modes; each at N = 64 and 128
+    want = {f"conv_tc_kernel<{ck}, float, {mode}, {nt}>" for ck, modes in ((64, (0, 2, 17, 19)), (32, (0, 1, 2, 3)))
+            for mode in modes for nt in (64, 128)}
+    assert set(tf) == want, sorted(tf)
     for n, r in tf.items():
         assert r["LDL"] == 0 and r["STL"] == 0, f"{n}: {r['LDL']} LDL / {r['STL']} STL"
         assert r["HGMMA"] > 0 and r["UTMALDG"] > 0, n
         assert r["USETMAXREG"] == 2, n
     hg = {f: lines for f, lines in _sass_by_function().items() if "conv_tc_kernel" in f}
     tf_mangled = [f for f in hg if re.search(r"conv_tc_kernelILi(64|32)EfLi", f)]
-    assert len(tf_mangled) == 20
+    assert len(tf_mangled) == 16
     for f in tf_mangled:
         assert hg[f] and all(re.search(r"HGMMA\.64x(64|128)x8\.F32\.TF32", l) for l in hg[f]), f
     for f, lines in hg.items():
