@@ -7,9 +7,10 @@
 // Per 16-wide x 8-tall output tile (persistent CTAs, the conv_tc_kernel warp layout: four consumer warpgroups as two
 // ping-pong teams of two, one producer warp):
 //   * Tiles.  The CTA's k-th tile is blockIdx.x + k * gridDim.x; team k & 1 computes it, in input box k & 1, with that
-//     box's own full / empty mbarrier pair.  The producer refills a box as soon as its team's conv2 wgmmas completed, so
-//     the next tile's load runs under the other team's MMAs.  x-paired blocks (dense 32-channel tensors,
-//     ACR_CONV_XPAIR) count the tile and the box in pixel pairs (a 32 x 8 pixel tile).
+//     box's own full / empty mbarrier pair.  The producer refills a box as soon as its team's conv2 wgmmas completed, and
+//     when it issues a box's load it also pulls the team's next box (tile k + 2) into L2, so that refill waits on L2, not
+//     on HBM.  x-paired blocks (dense 32-channel tensors, ACR_CONV_XPAIR) count the tile and the box in pixel pairs (a
+//     32 x 8 pixel tile).
 //   * Input: one TMA box {64 ch, 24-pixel pitch, 12 rows} from (x0-2, y0-2): a two-pixel halo, TMA's out-of-bounds zeros
 //     are conv1's padding.
 //   * conv1 over the 10 x 18 intermediate region (the tile plus conv2's one-pixel halo), "flat M": the pitch-24 box is a
@@ -21,9 +22,12 @@
 //     reads only feed the discarded flat row 10 and columns 18..23).
 //   * conv1 epilogue IN PLACE: once every conv1 wgmma of the team's tile has completed (a barrier over the team), bias +
 //     ReLU, rounded to 16 bits, is stored over the box in the 128B-swizzled K-major layout TMA would have written (16-byte
-//     chunk index ^= pixel & 7), 10 rows at pitch 24.  Pixels outside the image are stored as ZERO: they are conv2's
-//     padding.  Columns 18..23 are never read.  Then fence.proxy.async and a second team barrier: conv2's taps read rows
-//     written by the team's other warpgroup.
+//     chunk index ^= pixel & 7), with stmatrix: one instruction stores four 8-pixel x 16-byte fragments, so the
+//     epilogue issues 8 shared stores per thread instead of 32 (it runs while the other team streams wgmmas, which
+//     leave its instructions few issue and shared-memory slots).  Pixels outside the image are stored as ZERO: they are
+//     conv2's padding.  stmatrix writes whole M blocks, so flat row 10 and columns 18..23 get values too; conv2 never
+//     reads them.  Then fence.proxy.async and a second team barrier: conv2's taps read rows written by the team's other
+//     warpgroup.
 //   * conv2 reads the intermediate with the MODE_P1 addressing (one 8x8-pixel M block per warpgroup at pitch 24, taps =
 //     descriptor starts); once its wgmmas completed the box is handed back to the producer, then the conv2 epilogue
 //     (bias, residual from global, ReLU, NHWC stores).
@@ -66,6 +70,7 @@ static_assert(BLK_M_BLOCKS * 64 >= BLK_MID_ROWS * BLK_PITCH && (BLK_M_BLOCKS - 1
 static_assert(BLK_SLACK_PIX == 18 && BLK_BOX_STRIDE == 39936, "flat-M plan: the last M block reads 18 pixels past the box");
 static_assert(BLK_OFF_A % 1024 == 0 && BLK_BOX_STRIDE % 1024 == 0, "128B swizzle: every box starts on a 1024 B boundary");
 static_assert(BLK_MID_ROWS * BLK_PITCH * BLK_ROW_BYTES <= BLK_BOX_BYTES, "the intermediate fits in the box it overwrites");
+static_assert(BLK_M_BLOCKS * 64 <= BLK_PITCH * BLK_ROWS, "the conv1 epilogue's whole-block stores stay inside the box");
 static_assert(BLK_SMEM == 228160 && BLK_SMEM <= (size_t)SMEM_BUDGET,
               "fused-block shared-memory plan: 144 KB weights + two 1024-aligned boxes with slack + biases + barriers");
 static_assert(TILE_Y % BLK_TILE_Y == 0, "the 16-row super-tile precondition covers the 8-row tiles");
@@ -113,6 +118,19 @@ __device__ __forceinline__ void blk_conv(float* acc0, float* acc1, uint32_t a_lo
       blk_tap<T, XPAIR>(acc0, a_lo0 + off, hi_a, bt, hi_b, kx, first);
       if (NB == 2) blk_tap<T, XPAIR>(acc1, a_lo1 + off, hi_a, bt, hi_b, kx, first);
     }
+}
+
+// pull one TMA box into L2 (no shared-memory destination, no completion to wait for)
+__device__ __forceinline__ void tma_prefetch_l2_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];"
+               ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+
+// four 8x8 16-bit fragments (r_i = this thread's pair of fragment i) to shared memory; lane l gives the address of row
+// l & 7 of fragment l >> 3
+__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3) : "memory");
 }
 
 // wait on named barrier `id` when pred != 0; one asm statement, no branch between the wgmma groups
@@ -174,6 +192,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_block_kernel(const __grid_
       if (elect_one_sync()) {
         mbar_expect_tx(full_bar0 + 8 * bx, BLK_BOX_BYTES);
         tma_load_4d(a_base0 + (uint32_t)bx * BLK_BOX_STRIDE, &P.tmA, full_bar0 + 8 * bx, 0, x0 - 2, y0 - 2, n);
+        if (k + 2 < ntiles) {   // the box's next tile, into L2
+          const int t2 = tile + 2 * (int)gridDim.x, rem2 = t2 % P.tiles_per_img;
+          tma_prefetch_l2_4d(&P.tmA, 0, (rem2 % P.tiles_x) * TILE_X - 2, (rem2 / P.tiles_x) * BLK_TILE_Y - 2,
+                             t2 / P.tiles_per_img);
+        }
       }
       __syncwarp();
     }
@@ -208,30 +231,32 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_block_kernel(const __grid_
   auto turn_pre = [&](int s) { named_bar_sync_if(TEAM_BAR + team, 512, turn_exists(s - 1)); };
   auto turn_post = [&](int s) { named_bar_arrive_if(TEAM_BAR + (team ^ 1), 512, turn_exists(s + 1)); };
 
-  // conv1 epilogue of one M block, in place over the box
-  auto mid_store = [&](const float* acc, int blk, int y0, int x0, int n) {
+  // conv1 epilogue of one M block, in place over the box; bb[j] = conv1's bias of channels 8 j + cq, + 1
+  auto mid_store = [&](const float* acc, const float2* bb, int blk, int y0, int x0, int n) {
 #pragma unroll
     for (int r2 = 0; r2 < 2; ++r2) {
-      const int q = 64 * blk + 16 * wq + (lane >> 2) + 8 * r2;    // flat intermediate pixel
+      const int q = 64 * blk + 16 * wq + (lane >> 2) + 8 * r2;    // flat intermediate pixel of this thread's values
       const int r = q / BLK_PITCH, c = q - r * BLK_PITCH;
-      if (r >= BLK_MID_ROWS || c >= BLK_MID_COLS) continue;
       const int y = y0 - 1 + r, x = x0 - 1 + c;
-      const bool inside = y >= 0 && y < P.H && x >= 0 && x < P.W;
-      const bool keep = mid != nullptr && r >= 1 && r <= BLK_TILE_Y && c >= 1 && c <= TILE_X;
-      T* mp = keep ? mid + (((size_t)n * P.H + y) * P.W + x) * P.mid_stride : nullptr;
-      const uint32_t row = a_base + (uint32_t)q * BLK_ROW_BYTES;
+      const bool inside = r < BLK_MID_ROWS && c < BLK_MID_COLS && y >= 0 && y < P.H && x >= 0 && x < P.W;
+      uint32_t v[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const int ch = 8 * j + cq;
-        uint32_t v = 0u;
-        if (inside) {
-          float f0 = acc[4 * j + 2 * r2] + s_bias[ch], f1 = acc[4 * j + 2 * r2 + 1] + s_bias[ch + 1];
-          f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
-          v = pack2<T>(f0, f1);
-          if (keep) *reinterpret_cast<uint32_t*>(mp + ch) = v;
-        }
-        sts32(row + ((((uint32_t)j ^ ((uint32_t)q & 7u))) << 4) + (uint32_t)cq * 2u, v);
+        float f0 = acc[4 * j + 2 * r2] + bb[j].x, f1 = acc[4 * j + 2 * r2 + 1] + bb[j].y;
+        f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
+        v[j] = inside ? pack2<T>(f0, f1) : 0u;
       }
+      if (mid != nullptr && inside && r >= 1 && r <= BLK_TILE_Y && c >= 1 && c <= TILE_X) {
+        T* mp = mid + (((size_t)n * P.H + y) * P.W + x) * P.mid_stride + cq;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t*>(mp + 8 * j) = v[j];
+      }
+      // lane l stores row l & 7 of chunks 4 h + (l >> 3); that pixel's swizzle is l & 7
+      const uint32_t row = a_base + (uint32_t)(64 * blk + 16 * wq + 8 * r2 + (lane & 7)) * BLK_ROW_BYTES;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        stsm_x4(row + (((uint32_t)(4 * h + (lane >> 3)) ^ (uint32_t)(lane & 7)) << 4), v[4 * h], v[4 * h + 1], v[4 * h + 2],
+                v[4 * h + 3]);
     }
   };
 
@@ -252,8 +277,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_block_kernel(const __grid_
     wgmma_acc_fence<32>(acc0);
     wgmma_acc_fence<32>(acc1);
     named_bar_sync(BLK_BAR + team, 256);   // every conv1 wgmma of the tile has read the box: overwrite it
-    mid_store(acc0, blk0, y0, x0, n);
-    mid_store(acc1, blk1, y0, x0, n);
+    float2 bb[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) bb[j] = *reinterpret_cast<const float2*>(s_bias + 8 * j + cq);
+    mid_store(acc0, bb, blk0, y0, x0, n);
+    mid_store(acc1, bb, blk1, y0, x0, n);
     fence_proxy_async();                   // generic-proxy stores -> wgmma operand reads
     named_bar_sync(BLK_BAR + team, 256);
     // ---- conv2 over the intermediate, MODE_P1 addressing
