@@ -1,8 +1,8 @@
 // One HRNet BasicBlock (conv3x3-BN-ReLU, conv3x3-BN, + block input, ReLU) as ONE wgmma launch, sm_90a.
 //
 // Two conv_tc launches move five activation passes through HBM per block (read x, write y, read y, write the output,
-// read x again as the residual); this kernel moves two (read x, write the output; the residual re-read of the tile just
-// loaded hits L2).  The intermediate y never leaves shared memory.
+// read x again as the residual); this kernel moves two (read x, write the output; the residual is read from the input
+// box).  The intermediate y never leaves shared memory.
 //
 // Per 16-wide x 8-tall output tile (persistent CTAs, the conv_tc_kernel warp layout: four consumer warpgroups as two
 // ping-pong teams of two, one producer warp):
@@ -13,24 +13,28 @@
 //     32 x 8 pixel tile).
 //   * Input: one TMA box {64 ch, 24-pixel pitch, 12 rows} from (x0-2, y0-2): a two-pixel halo, TMA's out-of-bounds zeros
 //     are conv1's padding.
-//   * conv1 over the 10 x 18 intermediate region (the tile plus conv2's one-pixel halo), "flat M": the pitch-24 box is a
+//   * conv1 over the 10 x 18 intermediate region (the tile plus conv2's one-pixel halo), "flat": the pitch-24 box is a
 //     flat array of pixels and intermediate pixel p = r * 24 + c reads input pixel p + ky * 24 + kx for tap (ky, kx), a
-//     constant offset.  So every M = 64 block is 64 consecutive flat pixels (8 core groups of 8, SBO = 1024 B) and a tap
-//     is a descriptor start (ky * 24 + kx) * 128 B into the box -- an unaligned start, like MODE_P1 (the 128B swizzle
-//     follows the absolute address).  10 x 24 = 240 flat pixels take exactly the team's 4 M blocks; warpgroup w of the
-//     team owns blocks w and w + 2.  The last block reads up to 18 pixels past the box: a zeroed slack region (those
-//     reads only feed the discarded flat row 10 and columns 18..23).
+//     constant offset.  The resident weights ([tap][cout][64 ch], K-major) are the wgmma A operand, M = the 64 output
+//     channels, and N = 120 consecutive flat pixels are B (15 core groups of 8, SBO = 1024 B); a tap is a descriptor
+//     start (ky * 24 + kx) * 128 B into the box -- an unaligned start, like MODE_P1 (the 128B swizzle follows the
+//     absolute address).  10 x 24 = 240 flat pixels are exactly the team's two N ranges: warpgroup w of the team issues
+//     one m64n120k16 per tap and k-step over pixels [120 w, 120 w + 120).  The accumulator is the standalone conv's,
+//     transposed: each element is the same dot product over the same k-steps in the same order, and the tensor core
+//     reduces it the same way from either operand side (checked bit for bit on H100, bf16 and fp16).  Pixel 239 reads 2
+//     pixels past the box: a zeroed slack (those reads only feed flat columns 22..23, which conv2 never reads).
 //   * conv1 epilogue IN PLACE: once every conv1 wgmma of the team's tile has completed (a barrier over the team), bias +
 //     ReLU, rounded to 16 bits, is stored over the box in the 128B-swizzled K-major layout TMA would have written (16-byte
-//     chunk index ^= pixel & 7), with stmatrix: one instruction stores four 8-pixel x 16-byte fragments, so the
-//     epilogue issues 8 shared stores per thread instead of 32 (it runs while the other team streams wgmmas, which
-//     leave its instructions few issue and shared-memory slots).  Pixels outside the image are stored as ZERO: they are
-//     conv2's padding.  stmatrix writes whole M blocks, so flat row 10 and columns 18..23 get values too; conv2 never
-//     reads them.  Then fence.proxy.async and a second team barrier: conv2's taps read rows written by the team's other
-//     warpgroup.
+//     chunk index ^= pixel & 7), with stmatrix.trans: a fragment of 8 channels x 8 pixels, transposed, is those pixels'
+//     16-byte chunks, so a thread issues 8 shared stores for its 30 pixel pairs x 2 channels (the epilogue runs while
+//     the other team streams wgmmas, which leave its instructions few issue and shared-memory slots).  Pixels outside
+//     the image are stored as ZERO: they are conv2's padding; tiles whose 10 x 18 region lies inside the image skip the
+//     masks.  Flat columns 18..23 get values too; conv2 never reads them.  Then fence.proxy.async and a second team
+//     barrier: conv2's taps read rows written by the team's other warpgroup.
 //   * conv2 reads the intermediate with the MODE_P1 addressing (one 8x8-pixel M block per warpgroup at pitch 24, taps =
 //     descriptor starts); once its wgmmas completed the box is handed back to the producer, then the conv2 epilogue
-//     (bias, residual from global, ReLU, NHWC stores).
+//     (bias, residual, ReLU, NHWC stores).  The residual is read from the box into registers (ldmatrix) before the conv1
+//     epilogue overwrites it.
 //   * Ping-pong: the teams take turns issuing one group of wgmmas each (a tile's conv1, or its conv2), so the turns run
 //     team 0 conv1, team 1 conv1, team 0 conv2, team 1 conv2, team 0 conv1 of its next tile, ...  A team holds the turn
 //     only while it issues and hands it over before it waits for its wgmmas, so its waits, barriers and epilogues run
@@ -43,9 +47,12 @@
 //   * Bit-identical to the two conv_tc launches: every accumulator sums its taps and k-steps in the standalone order
 //     (ky-major, kx 0,1,2; x-paired: kx 1,0,2, side taps as full-width MMAs over zero weight quarters), the epilogues do
 //     the same float operations, and the intermediate is rounded to 16 bits in both paths.
-//   * `mid` (optional): conv1's output is also stored for the tile's own 16x8 pixels, so an observable intermediate
-//     (teacher-forced checks, kept tensors) is still written.
+//   * `mid` (optional): conv1's output for the tile's own 16x8 pixels is also copied from the box to global (16-byte
+//     chunks, unswizzled) while conv2's wgmmas run, so an observable intermediate (teacher-forced checks, kept tensors)
+//     is still written.
 #pragma once
+#include <type_traits>
+
 #include "conv_tc.cuh"
 
 namespace acr {
@@ -56,8 +63,8 @@ constexpr int BLK_MID_ROWS = BLK_TILE_Y + 2, BLK_MID_COLS = TILE_X + 2;   // int
 constexpr uint32_t BLK_ROW_BYTES = 128;                            // 64 16-bit channels
 constexpr uint32_t BLK_W_BYTES = 9u * 64u * BLK_ROW_BYTES;         // one conv's resident weights: 9 taps x [64][64]
 constexpr uint32_t BLK_BOX_BYTES = (uint32_t)BLK_PITCH * BLK_ROWS * BLK_ROW_BYTES;
-constexpr int BLK_M_BLOCKS = 4;                                    // conv1 M blocks of a tile: 2 per warpgroup of the team
-constexpr int BLK_SLACK_PIX = BLK_M_BLOCKS * 64 + 2 * BLK_PITCH + 2 - BLK_PITCH * BLK_ROWS;
+constexpr int BLK_CONV1_N = 120;   // conv1 flat pixels per warpgroup: the N of its m64n120k16 (A = the 64 output channels)
+constexpr int BLK_SLACK_PIX = 2 * BLK_CONV1_N + 2 * BLK_PITCH + 2 - BLK_PITCH * BLK_ROWS;
 constexpr uint32_t BLK_SLACK_BYTES = (uint32_t)BLK_SLACK_PIX * BLK_ROW_BYTES;
 constexpr uint32_t BLK_BOX_STRIDE = (BLK_BOX_BYTES + BLK_SLACK_BYTES + 1023u) & ~1023u;   // box 1 starts 1024-aligned
 constexpr uint32_t BLK_OFF_B2 = BLK_W_BYTES;
@@ -65,13 +72,12 @@ constexpr uint32_t BLK_OFF_A = 2 * BLK_W_BYTES;                    // box t at B
 constexpr uint32_t BLK_OFF_BIAS = BLK_OFF_A + BLK_BOX_STRIDE + BLK_BOX_BYTES + BLK_SLACK_BYTES;
 constexpr uint32_t BLK_OFF_BAR = BLK_OFF_BIAS + 2 * 64 * 4;
 constexpr size_t BLK_SMEM = 1024 /*alignment slack*/ + BLK_OFF_BAR + 64;
-static_assert(BLK_M_BLOCKS * 64 >= BLK_MID_ROWS * BLK_PITCH && (BLK_M_BLOCKS - 1) * 64 < BLK_MID_ROWS * BLK_PITCH,
-              "flat-M plan: 4 M blocks of 64 cover the 240 flat intermediate pixels, none discarded");
-static_assert(BLK_SLACK_PIX == 18 && BLK_BOX_STRIDE == 39936, "flat-M plan: the last M block reads 18 pixels past the box");
+static_assert(2 * BLK_CONV1_N == BLK_MID_ROWS * BLK_PITCH && BLK_CONV1_N % BLK_PITCH == 0 && BLK_CONV1_N % 16 == 8,
+              "flat conv1: the team's two N = 120 ranges are the 240 flat intermediate pixels, 5 whole rows each");
+static_assert(BLK_SLACK_PIX == 2 && BLK_BOX_STRIDE == 37888, "flat conv1: pixel 239 reads 2 pixels past the box");
 static_assert(BLK_OFF_A % 1024 == 0 && BLK_BOX_STRIDE % 1024 == 0, "128B swizzle: every box starts on a 1024 B boundary");
 static_assert(BLK_MID_ROWS * BLK_PITCH * BLK_ROW_BYTES <= BLK_BOX_BYTES, "the intermediate fits in the box it overwrites");
-static_assert(BLK_M_BLOCKS * 64 <= BLK_PITCH * BLK_ROWS, "the conv1 epilogue's whole-block stores stay inside the box");
-static_assert(BLK_SMEM == 228160 && BLK_SMEM <= (size_t)SMEM_BUDGET,
+static_assert(BLK_SMEM == 224064 && BLK_SMEM <= (size_t)SMEM_BUDGET,
               "fused-block shared-memory plan: 144 KB weights + two 1024-aligned boxes with slack + biases + barriers");
 static_assert(TILE_Y % BLK_TILE_Y == 0, "the 16-row super-tile precondition covers the 8-row tiles");
 constexpr int BLK_BAR = 1;   // named barrier BLK_BAR + t over the 256 threads of team t
@@ -81,42 +87,42 @@ struct ConvBlockParams {
   CUtensorMap tmB1, tmB2;   // packed weights of conv1 / conv2 [64][9 * 64], box {64, 64}
   const float* bias1;
   const float* bias2;
-  const void* res;          // the block input again (residual of conv2)
   void* out;
   void* mid;                // conv1's output buffer, or nullptr when nothing reads it
-  int res_stride, out_stride, mid_stride;
+  int out_stride, mid_stride;
   int H, W, tiles_x, tiles_per_img, total_tiles;   // 16 x 8 tiles
 };
 
-// the wgmmas of one tap of one accumulator (x-paired side taps: the two k-steps of their K half, see conv_tc_kernel)
-template <typename T, bool XPAIR>
+// the wgmmas of one tap, D[64][N] += A * B (x-paired side taps: the two k-steps of their K half, see conv_tc_kernel)
+template <typename T, bool XPAIR, int N>
 __device__ __forceinline__ void blk_tap(float* acc, uint32_t a_lo, uint32_t hi_a, uint32_t b_lo, uint32_t hi_b, int kx,
                                         bool first) {
   if (XPAIR && kx != 1) {
     const int ks0 = kx == 0 ? 2 : 0;
 #pragma unroll
-    for (int ks = ks0; ks < ks0 + 2; ++ks) wgmma_m64k16<64, T>(acc, desc_lohi(a_lo + ks * 2, hi_a), desc_lohi(b_lo + ks * 2, hi_b));
+    for (int ks = ks0; ks < ks0 + 2; ++ks) wgmma_m64k16<N, T>(acc, desc_lohi(a_lo + ks * 2, hi_a), desc_lohi(b_lo + ks * 2, hi_b));
   } else {
 #pragma unroll
     for (int ks = 0; ks < 4; ++ks)
-      wgmma_m64k16<64, T>(acc, desc_lohi(a_lo + ks * 2, hi_a), desc_lohi(b_lo + ks * 2, hi_b), (first && ks == 0) ? 0u : 1u);
+      wgmma_m64k16<N, T>(acc, desc_lohi(a_lo + ks * 2, hi_a), desc_lohi(b_lo + ks * 2, hi_b), (first && ks == 0) ? 0u : 1u);
   }
 }
 
-// all nine taps of NB accumulators (NB = 1 or 2), tap-interleaved; a_lo[i] = tap (0,0) of accumulator i
-template <typename T, bool XPAIR, int NB>
-__device__ __forceinline__ void blk_conv(float* acc0, float* acc1, uint32_t a_lo0, uint32_t a_lo1, uint32_t hi_a,
-                                         uint32_t a_row16, uint32_t b_lo, uint32_t hi_b) {
+// all nine taps of one accumulator; px_lo = the pixels of tap (0,0), w_lo = the weights of tap 0.  W_AS_A (conv1): the
+// weights are A (M = the 64 output channels) and BLK_CONV1_N pixels are B; else (conv2) 64 pixels are A and the weights B
+template <typename T, bool XPAIR, bool W_AS_A>
+__device__ __forceinline__ void blk_conv(float* acc, uint32_t px_lo, uint32_t hi_px, uint32_t w_lo, uint32_t hi_w) {
+  constexpr uint32_t pix16 = BLK_ROW_BYTES >> 4, row16 = (uint32_t)BLK_PITCH * pix16;
 #pragma unroll
   for (int ky = 0; ky < 3; ++ky)
 #pragma unroll
     for (int i = 0; i < 3; ++i) {
       const int kx = XPAIR ? (i == 0 ? 1 : (i == 1 ? 0 : 2)) : i;
-      const uint32_t off = (uint32_t)ky * a_row16 + (uint32_t)kx * (BLK_ROW_BYTES >> 4);
-      const uint32_t bt = b_lo + (uint32_t)(ky * 3 + kx) * ((64u * BLK_ROW_BYTES) >> 4);
+      const uint32_t px = px_lo + (uint32_t)ky * row16 + (uint32_t)kx * pix16;
+      const uint32_t wt = w_lo + (uint32_t)(ky * 3 + kx) * ((64u * BLK_ROW_BYTES) >> 4);
       const bool first = ky == 0 && i == 0;
-      blk_tap<T, XPAIR>(acc0, a_lo0 + off, hi_a, bt, hi_b, kx, first);
-      if (NB == 2) blk_tap<T, XPAIR>(acc1, a_lo1 + off, hi_a, bt, hi_b, kx, first);
+      if constexpr (W_AS_A) blk_tap<T, XPAIR, BLK_CONV1_N>(acc, wt, hi_w, px, hi_px, kx, first);
+      else blk_tap<T, XPAIR, 64>(acc, px, hi_px, wt, hi_w, kx, first);
     }
 }
 
@@ -126,11 +132,25 @@ __device__ __forceinline__ void tma_prefetch_l2_4d(const CUtensorMap* map, int c
                ::"l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
 }
 
-// four 8x8 16-bit fragments (r_i = this thread's pair of fragment i) to shared memory; lane l gives the address of row
-// l & 7 of fragment l >> 3
-__device__ __forceinline__ void stsm_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
-  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
-               "r"(r3) : "memory");
+// 8x8 16-bit fragments (r_i = this thread's pair of fragment i: row lane >> 2, columns 2 (lane & 3) + {0, 1}) to shared
+// memory TRANSPOSED: column c of fragment i goes to the 16 bytes at the address of lane 8 i + c
+__device__ __forceinline__ void stsm_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3) : "memory");
+}
+__device__ __forceinline__ void stsm_x2_trans(uint32_t addr, uint32_t r0, uint32_t r1) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x2.trans.shared.b16 [%0], {%1, %2};" ::"r"(addr), "r"(r0), "r"(r1) : "memory");
+}
+// four 8x8 16-bit fragments from shared memory (r_i: row lane >> 2, columns 2 (lane & 3) + {0, 1} of fragment i); lane l
+// gives the address of row l & 7 of fragment l >> 3
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
+               : "r"(addr) : "memory");
+}
+__device__ __forceinline__ uint4 lds128(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
 }
 
 // wait on named barrier `id` when pred != 0; one asm statement, no branch between the wgmma groups
@@ -218,46 +238,57 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_block_kernel(const __grid_
   const uint32_t full_bar = full_bar0 + 8 * team, empty_bar = empty_bar0 + 8 * team;
   const uint32_t a_lo = ((a_base >> 4) & 0x3FFF) | lo_flags;
   const uint32_t b1_lo = ((b1_base >> 4) & 0x3FFF) | lo_flags, b2_lo = ((b2_base >> 4) & 0x3FFF) | lo_flags;
-  constexpr uint32_t pix16 = BLK_ROW_BYTES >> 4, row16 = (uint32_t)BLK_PITCH * pix16;
-  const int blk0 = w, blk1 = w + 2;                                  // conv1 M blocks of this warpgroup
+  constexpr uint32_t pix16 = BLK_ROW_BYTES >> 4;
   const int cq = 2 * (lane & 3);
   const uint32_t is_lane0 = lane == 0 ? 1u : 0u;
-  const T* res = reinterpret_cast<const T*>(P.res);
   T* out = reinterpret_cast<T*>(P.out);
   T* mid = reinterpret_cast<T*>(P.mid);
-  float acc0[32], acc1[32];
+  // conv1's accumulator is transposed (M = channels): this thread holds channels ch1 and ch1 + 8 of the warpgroup's flat
+  // pixels 120 w + 8 j + cq + {0, 1}, j < 15, which are row 5 w + j / 3, columns 8 (j % 3) + cq + {0, 1}
+  const int ch1 = 16 * wq + (lane >> 2);
+  const float bias1_lo = s_bias[ch1], bias1_hi = s_bias[ch1 + 8];
+  // stmatrix.trans of the fragments (channels 8 h.., pixels 8 j..) stores those 8 pixels' 16-byte chunk 2 wq + h.  For
+  // fragment pair t, lane l gives the row of pixel 8 (2 t + (l >> 4)) + (l & 7), chunk 2 wq + ((l >> 3) & 1) ^ (l & 7)
+  const uint32_t epi_row = a_base + (uint32_t)(BLK_CONV1_N * w + 8 * (lane >> 4) + (lane & 7)) * BLK_ROW_BYTES +
+                           (((uint32_t)(2 * wq + ((lane >> 3) & 1)) ^ (uint32_t)(lane & 7)) << 4);
+  float acc1[BLK_CONV1_N / 2], acc2[32];
   // turn s exists when the CTA has its tile (see the header); turn_pre / turn_post: wait for the turn, hand it on
   auto turn_exists = [&](int s) -> uint32_t { return (s >= 0 && 2 * (s >> 2) + (s & 1) < ntiles) ? 1u : 0u; };
   auto turn_pre = [&](int s) { named_bar_sync_if(TEAM_BAR + team, 512, turn_exists(s - 1)); };
   auto turn_post = [&](int s) { named_bar_arrive_if(TEAM_BAR + (team ^ 1), 512, turn_exists(s + 1)); };
 
-  // conv1 epilogue of one M block, in place over the box; bb[j] = conv1's bias of channels 8 j + cq, + 1
-  auto mid_store = [&](const float* acc, const float2* bb, int blk, int y0, int x0, int n) {
+  // conv1 epilogue in place over the box: bias + ReLU, rounded to 16 bits.  `masked` (std::true_type) zeroes the pixels
+  // outside the image (conv2's padding); columns 18..23 are never read, so an interior tile masks nothing.
+  auto conv1_epilogue = [&](auto masked, int y0, int x0) {
+    uint32_t colm[3], rowm[5];   // per j % 3: the (pixel, pixel + 1) halves of a packed word; per j / 3: the row
+    if constexpr (decltype(masked)::value) {
 #pragma unroll
-    for (int r2 = 0; r2 < 2; ++r2) {
-      const int q = 64 * blk + 16 * wq + (lane >> 2) + 8 * r2;    // flat intermediate pixel of this thread's values
-      const int r = q / BLK_PITCH, c = q - r * BLK_PITCH;
-      const int y = y0 - 1 + r, x = x0 - 1 + c;
-      const bool inside = r < BLK_MID_ROWS && c < BLK_MID_COLS && y >= 0 && y < P.H && x >= 0 && x < P.W;
-      uint32_t v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float f0 = acc[4 * j + 2 * r2] + bb[j].x, f1 = acc[4 * j + 2 * r2 + 1] + bb[j].y;
-        f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
-        v[j] = inside ? pack2<T>(f0, f1) : 0u;
+      for (int jm = 0; jm < 3; ++jm) {
+        const int x = x0 - 1 + 8 * jm + cq;
+        colm[jm] = (x >= 0 && x < P.W ? 0xFFFFu : 0u) | (x + 1 >= 0 && x + 1 < P.W ? 0xFFFF0000u : 0u);
       }
-      if (mid != nullptr && inside && r >= 1 && r <= BLK_TILE_Y && c >= 1 && c <= TILE_X) {
-        T* mp = mid + (((size_t)n * P.H + y) * P.W + x) * P.mid_stride + cq;
 #pragma unroll
-        for (int j = 0; j < 8; ++j) *reinterpret_cast<uint32_t*>(mp + 8 * j) = v[j];
+      for (int jr = 0; jr < 5; ++jr) {
+        const int y = y0 - 1 + (BLK_CONV1_N / BLK_PITCH) * w + jr;
+        rowm[jr] = y >= 0 && y < P.H ? ~0u : 0u;
       }
-      // lane l stores row l & 7 of chunks 4 h + (l >> 3); that pixel's swizzle is l & 7
-      const uint32_t row = a_base + (uint32_t)(64 * blk + 16 * wq + 8 * r2 + (lane & 7)) * BLK_ROW_BYTES;
-#pragma unroll
-      for (int h = 0; h < 2; ++h)
-        stsm_x4(row + (((uint32_t)(4 * h + (lane >> 3)) ^ (uint32_t)(lane & 7)) << 4), v[4 * h], v[4 * h + 1], v[4 * h + 2],
-                v[4 * h + 3]);
     }
+    uint32_t v[2][BLK_CONV1_N / 8];
+#pragma unroll
+    for (int j = 0; j < BLK_CONV1_N / 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float b = h ? bias1_hi : bias1_lo;
+        float f0 = acc1[4 * j + 2 * h] + b, f1 = acc1[4 * j + 2 * h + 1] + b;
+        f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f);
+        v[h][j] = pack2<T>(f0, f1);
+        if constexpr (decltype(masked)::value) v[h][j] &= colm[j % 3] & rowm[j / 3];
+      }
+#pragma unroll
+    for (int t = 0; t < BLK_CONV1_N / 16; ++t)
+      stsm_x4_trans(epi_row + (uint32_t)t * 16u * BLK_ROW_BYTES, v[0][2 * t], v[1][2 * t], v[0][2 * t + 1], v[1][2 * t + 1]);
+    stsm_x2_trans(epi_row + (uint32_t)(BLK_CONV1_N / 16) * 16u * BLK_ROW_BYTES, v[0][BLK_CONV1_N / 8 - 1],
+                  v[1][BLK_CONV1_N / 8 - 1]);
   };
 
   for (int k = team; k < ntiles; k += 2) {
@@ -266,52 +297,67 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv_block_kernel(const __grid_
     const int y0 = (rem / P.tiles_x) * BLK_TILE_Y, x0 = (rem % P.tiles_x) * TILE_X;
     const int s = 2 * k - team;   // this tile's conv1 turn; its conv2 turn is s + 2
     mbar_wait_parity(full_bar, (uint32_t)(k >> 1) & 1u);
-    // ---- conv1 over the flat 10 x 24 region
+    // ---- conv1 over the flat 10 x 24 region: the weights are A, this warpgroup's 120 flat pixels are B
     turn_pre(s);
     wgmma_fence();
-    blk_conv<T, XPAIR, 2>(acc0, acc1, a_lo + (uint32_t)(64 * blk0) * pix16, a_lo + (uint32_t)(64 * blk1) * pix16, hi_flat, row16,
-                          b1_lo, hi_b);
+    blk_conv<T, XPAIR, true>(acc1, a_lo + (uint32_t)(BLK_CONV1_N * w) * pix16, hi_flat, b1_lo, hi_b);
     wgmma_commit();
     turn_post(s);
     wgmma_wait<0>();
-    wgmma_acc_fence<32>(acc0);
-    wgmma_acc_fence<32>(acc1);
-    named_bar_sync(BLK_BAR + team, 256);   // every conv1 wgmma of the tile has read the box: overwrite it
-    float2 bb[8];
+    wgmma_acc_fence<BLK_CONV1_N / 2>(acc1);
+    // conv2's residual is the block input at the tile's own pixels, which the box holds (rows 2 wq + r2 + 2, columns
+    // 8 w + 2 + (lane >> 2)) until the epilogue overwrites it.  An 8-pixel x 8-channel ldmatrix fragment is the
+    // accumulator's layout: rv[r2][j] = channels 8 j + cq, + 1.  From global, each tile's residual loads took thousands
+    // of cycles to land, and the team's next tile waited for them.
+    uint32_t rv[2][8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) bb[j] = *reinterpret_cast<const float2*>(s_bias + 8 * j + cq);
-    mid_store(acc0, bb, blk0, y0, x0, n);
-    mid_store(acc1, bb, blk1, y0, x0, n);
+    for (int r2 = 0; r2 < 2; ++r2) {
+      const uint32_t q = (uint32_t)((2 * wq + r2 + 2) * BLK_PITCH + HALF_X * w + 2 + (lane & 7));
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        ldsm_x4(a_base + q * BLK_ROW_BYTES + (((uint32_t)(4 * h + (lane >> 3)) ^ (q & 7u)) << 4), rv[r2][4 * h],
+                rv[r2][4 * h + 1], rv[r2][4 * h + 2], rv[r2][4 * h + 3]);
+    }
+    named_bar_sync(BLK_BAR + team, 256);   // every conv1 wgmma and residual read of the tile is done: overwrite the box
+    if (x0 >= 1 && x0 + BLK_MID_COLS - 1 <= P.W && y0 >= 1 && y0 + BLK_MID_ROWS - 1 <= P.H)
+      conv1_epilogue(std::false_type{}, y0, x0);
+    else
+      conv1_epilogue(std::true_type{}, y0, x0);
     fence_proxy_async();                   // generic-proxy stores -> wgmma operand reads
     named_bar_sync(BLK_BAR + team, 256);
     // ---- conv2 over the intermediate, MODE_P1 addressing
     turn_pre(s + 2);
     wgmma_fence();
-    blk_conv<T, XPAIR, 1>(acc0, acc0, a_lo + (uint32_t)w * 8u * pix16, 0u, hi_p1, row16, b2_lo, hi_b);
+    blk_conv<T, XPAIR, false>(acc2, a_lo + (uint32_t)w * 8u * pix16, hi_p1, b2_lo, hi_b);
     wgmma_commit();
     turn_post(s + 2);
-    // the residual (conv2's epilogue) is loaded while conv2's wgmmas run: all 16 loads in flight at once, where loads
-    // interleaved with the output stores would each wait out an L2 round trip
-    const int oy0 = y0 + 2 * wq, ox = x0 + w * HALF_X + (lane >> 2);
-    uint32_t rv[2][8];
+    if (mid != nullptr) {   // the tile's own 16 x 8 intermediate pixels: 16-byte chunks, unswizzled, from the box
+      const int tt = 128 * w + (threadIdx.x & 127);
 #pragma unroll
-    for (int r2 = 0; r2 < 2; ++r2) {
-      const T* rp = res + (((size_t)n * P.H + oy0 + r2) * P.W + ox) * P.res_stride;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) rv[r2][j] = *reinterpret_cast<const uint32_t*>(rp + 8 * j + cq);
+      for (int i = 0; i < 4; ++i) {
+        const int e = tt + 256 * i, pix = e >> 3, g = e & 7;
+        const int r = 1 + pix / TILE_X, c = 1 + pix % TILE_X, q = r * BLK_PITCH + c;
+        const int y = y0 - 1 + r, x = x0 - 1 + c;
+        const uint4 u = lds128(a_base + (uint32_t)q * BLK_ROW_BYTES + (((uint32_t)g ^ (uint32_t)(q & 7)) << 4));
+        if (y < P.H && x < P.W) {   // 4-byte stores: the buffer's pixel stride is only known to be even
+          uint32_t* mp = reinterpret_cast<uint32_t*>(mid + (((size_t)n * P.H + y) * P.W + x) * P.mid_stride + 8 * g);
+          mp[0] = u.x; mp[1] = u.y; mp[2] = u.z; mp[3] = u.w;
+        }
+      }
     }
     wgmma_wait<0>();
-    wgmma_acc_fence<32>(acc0);
+    wgmma_acc_fence<32>(acc2);
     __syncwarp();
     mbar_arrive_if(empty_bar, is_lane0);   // the box is free: the team's next tile loads under the other team's MMAs
     // ---- conv2 epilogue: + bias + residual, ReLU
+    const int oy0 = y0 + 2 * wq, ox = x0 + w * HALF_X + (lane >> 2);
 #pragma unroll
     for (int r2 = 0; r2 < 2; ++r2) {
       T* op = out + (((size_t)n * P.H + oy0 + r2) * P.W + ox) * P.out_stride;
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const int c = 8 * j + cq;
-        float f0 = acc0[4 * j + 2 * r2] + s_bias[64 + c], f1 = acc0[4 * j + 2 * r2 + 1] + s_bias[64 + c + 1];
+        float f0 = acc2[4 * j + 2 * r2] + s_bias[64 + c], f1 = acc2[4 * j + 2 * r2 + 1] + s_bias[64 + c + 1];
         float x0f, x1f;
         unpack2<T>(rv[r2][j], x0f, x1f);
         f0 += x0f; f1 += x1f;

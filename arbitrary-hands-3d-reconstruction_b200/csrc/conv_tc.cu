@@ -253,8 +253,8 @@ int conv_block_prepare(const ConvArgs& a1, const ConvArgs& a2, int act_dtype, in
   }
   if (rc) { delete pl; return rc; }
   p.bias1 = a1.bias; p.bias2 = a2.bias;
-  p.res = a2.res.ptr; p.out = a2.out.ptr; p.mid = store_mid ? a1.out.ptr : nullptr;
-  p.res_stride = a2.res.pix_stride; p.out_stride = a2.out.pix_stride; p.mid_stride = a1.out.pix_stride;
+  p.out = a2.out.ptr; p.mid = store_mid ? a1.out.ptr : nullptr;   // the residual is the input box (checked above)
+  p.out_stride = a2.out.pix_stride; p.mid_stride = a1.out.pix_stride;
   p.H = H; p.W = W;
   p.tiles_x = W / TILE_X; p.tiles_per_img = p.tiles_x * (H / BLK_TILE_Y);   // 16 x 8 tiles
   p.total_tiles = p.tiles_per_img * a1.batch;

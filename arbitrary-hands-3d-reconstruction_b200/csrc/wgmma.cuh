@@ -186,6 +186,27 @@ __device__ __forceinline__ void wgmma_m64n112k16(float* d, uint64_t da, uint64_t
         : "l"(da), "l"(db), "r"(scale_d));
 }
 
+// D[64][120] += A * B (A and B K-major)
+template <typename T>
+__device__ __forceinline__ void wgmma_m64n120k16(float* d, uint64_t da, uint64_t db, uint32_t scale_d = 1) {
+  if constexpr (IsBf16<T>::value)
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %62, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n120k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59}, "
+        "%60, %61, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59])
+        : "l"(da), "l"(db), "r"(scale_d));
+  else
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %62, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n120k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59}, "
+        "%60, %61, p, 1, 1, 0, 0;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59])
+        : "l"(da), "l"(db), "r"(scale_d));
+}
+
 // D[64][128] += A * B (A and B K-major)
 template <typename T>
 __device__ __forceinline__ void wgmma_m64n128k16(float* d, uint64_t da, uint64_t db, uint32_t scale_d = 1) {
@@ -316,11 +337,12 @@ __device__ __forceinline__ void wgmma_m64n128k8_tf32(float* d, uint64_t da, uint
       : "l"(da), "l"(db), "r"(scale_d));
 }
 
-// D[64][N] (+)= A * B for a compile-time N (a multiple of 16, <= 128): 32 bytes of K per operand row, i.e. one k16 step of
-// 16-bit operands (bf16 / f16) or one k8 step of fp32 operands, which the tensor cores read as tf32 (T = float)
+// D[64][N] (+)= A * B for a compile-time N (a multiple of 16, <= 128, or 120 for 16-bit operands): 32 bytes of K per
+// operand row, i.e. one k16 step of 16-bit operands (bf16 / f16) or one k8 step of fp32 operands, which the tensor cores
+// read as tf32 (T = float)
 template <int N, typename T>
 __device__ __forceinline__ void wgmma_m64k16(float* d, uint64_t da, uint64_t db, uint32_t scale_d = 1) {
-  static_assert(N % 16 == 0 && N >= 16 && N <= 128, "wgmma_m64k16: N");
+  static_assert((N % 16 == 0 && N >= 16 && N <= 128) || (N == 120 && !IsF32<T>::value), "wgmma_m64k16: N");
   if constexpr (IsF32<T>::value) {   // fp32 storage: ONE k8 tf32 step, the same 32 bytes of K per operand row
     if constexpr (N == 16) wgmma_m64n16k8_tf32(d, da, db, scale_d);
     else if constexpr (N == 32) wgmma_m64n32k8_tf32(d, da, db, scale_d);
@@ -337,6 +359,7 @@ __device__ __forceinline__ void wgmma_m64k16(float* d, uint64_t da, uint64_t db,
   else if constexpr (N == 80) wgmma_m64n80k16<T>(d, da, db, scale_d);
   else if constexpr (N == 96) wgmma_m64n96k16<T>(d, da, db, scale_d);
   else if constexpr (N == 112) wgmma_m64n112k16<T>(d, da, db, scale_d);
+  else if constexpr (N == 120) wgmma_m64n120k16<T>(d, da, db, scale_d);
   else wgmma_m64n128k16<T>(d, da, db, scale_d);
 }
 

@@ -59,8 +59,9 @@ class ClockSampler(threading.Thread):
 def conv_classes(recs, batch, blocks=(), bottlenecks=()):
     """[(key, [rec indices], GFLOP, algorithmic MB, weights KB, issued GFLOP)] of the conv launches, in plan order of first
     use.  `blocks`: first records of the BasicBlocks that run as one fused launch (csrc/conv_block.cuh), a class of their
-    own (k "3+3"): FLOP of both convs, bytes in + out, and the issued FLOP of the fused kernel (conv1 runs 8 M blocks of 64
-    flat rows per 16x16 tile, 2x its pixels; the x-paired form issues its side taps at full width, 4/3).
+    own (k "3+3"): FLOP of both convs, bytes in + out, and the issued FLOP of the fused kernel (conv1 runs two N = 120
+    ranges of flat pixels per 16x8 tile, 240 / 128 of its pixels; the x-paired form issues its side taps at full width,
+    4/3).
     `bottlenecks`: first records of the Bottlenecks that run as one fused launch (csrc/conv_bottleneck.cuh), a class of
     their own (k "1+3+1", cin = the block input's channels): FLOP of the three convs, bytes in + residual (when it is not
     the input) + out, and the issued FLOP (conv1 runs 4 M blocks of 64 flat rows per 16x8 tile, 2x its pixels)."""
@@ -91,7 +92,7 @@ def conv_classes(recs, batch, blocks=(), bottlenecks=()):
             a[1] += gflop
             a[2] += batch * (x.H * x.W * x.C + y.H * y.W * y.C) * 2 / 1e6
             a[3] = 2 * y.C * x.C * 9 * 2 / 1024
-            a[4] += gflop * 1.5 * (4 / 3 if x.C == 32 else 1)
+            a[4] += gflop * (240 / 128 + 1) / 2 * (4 / 3 if x.C == 32 else 1)   # conv1 240 / 128, conv2 exact
             continue
         cin = 109 if "fold_side" in at else (27 if "stem" in at else x.C)   # real input channels of the GEMM
         deconv = bool(at.get("deconv"))
