@@ -4,9 +4,10 @@
 // Work split.  A frame's entropy-coded segment is cut into chunks of ACR_B200_JPEG_CHUNK raw bytes, one thread
 // each.  A decoder state is (position, z, c): the raw byte and bit of the next code, the coefficient index of the
 // block being decoded (0 = its DC is next) and the block's slot in the MCU.  Positions are raw offsets in the
-// segment: byte stuffing (FF 00) is skipped when bits are read, and a restart marker is crossed when a decoder at
-// a code boundary finds nothing but padding ones before it.  A chunk's work is every code that starts at a
-// position before the chunk's end; its end state is the first code boundary at or past that end.
+// segment: byte stuffing (FF 00) is skipped when bits are read, and a restart marker, with any FF fill bytes before
+// it, is crossed when a decoder at a code boundary finds nothing but padding ones before it.  A chunk's work is
+// every code that starts at a position before the chunk's end; its end state is the first code boundary at or past
+// that end.
 //
 //   jpeg_spec_kernel   self-synchronising speculative decoding (Weissenberger & Schmidt, ICPP 2018): the thread of
 //                      chunk j guesses a code boundary at the start of chunk j-1 (z = c = 0), decodes through it
@@ -210,16 +211,24 @@ __device__ __forceinline__ void run(Decoder& d, const acr_b200_jpeg_frame& f, in
     const uint32_t w = d.peek(avail, stop);
     if (avail < 8 && (avail == 0 || (w >> (32 - avail)) == (1u << avail) - 1)) {   // only padding before a marker
       if (d.z != 0 || d.c != 0) { d.fail(s, ACR_B200_JPEG_TRUNCATED); continue; }
-      if (stop >= d.len) { d.flags |= ST_DONE; break; }
-      const int m = stop + 1 < d.len ? d.seg[stop + 1] : 0;
-      if (m < 0xD0 || m > 0xD7) { d.fail(s, stop + 1 < d.len ? ACR_B200_JPEG_BAD_MARKER : ACR_B200_JPEG_TRUNCATED); continue; }
+      // a marker may follow any number of FF fill bytes (T.81 B.1.1.2); fill bytes up to the segment's end
+      // precede its EOI
+      int q = stop;
+      while (q + 1 < d.len && d.seg[q + 1] == 0xFF) ++q;
+      if (q + 1 >= d.len) { d.flags |= ST_DONE; break; }
+      const int m = d.seg[q + 1];
+      if (m < 0xD0 || m > 0xD7) {   // resume past the fill run: a decoder crosses it once
+        d.b = q;
+        d.fail(s, ACR_B200_JPEG_BAD_MARKER);
+        continue;
+      }
       if (WRITE) {   // the interval before must be `restart` whole MCUs, and the marker the next in sequence
         const int next = st->cur + 1, per = f.restart * f.bpm;
         if (per == 0 || next == 0 || next % per != 0 || ((next / per - 1) & 7) != m - 0xD0)
           s.err |= ACR_B200_JPEG_BAD_RESTART;
         st->pred[0] = st->pred[1] = st->pred[2] = 0;
       }
-      d.b = stop + 2;
+      d.b = q + 2;
       d.o = 0;
       s.nres += 1;
       s.dc[0] = s.dc[1] = s.dc[2] = 0;
@@ -302,7 +311,9 @@ constexpr int SYNC_THREADS = 512;
 
 __device__ __forceinline__ bool same(int2 p, int2 q) { return p.x == q.x && p.y == q.y; }
 
-__global__ void __launch_bounds__(SYNC_THREADS) jpeg_sync_kernel(Args a) {
+// one CTA per frame, so occupancy does not matter: min blocks 1 keeps ptxas from capping the registers at 32 and
+// spilling the decoder state to local memory
+__global__ void __launch_bounds__(SYNC_THREADS, 1) jpeg_sync_kernel(Args a) {
   const acr_b200_jpeg_frame& f = a.frames[blockIdx.x];
   const int tid = threadIdx.x;
   if (f.ncomp == 0) {   // decoded elsewhere (host fallback)

@@ -26,7 +26,9 @@ F_1_961, F_2_053, F_2_562, F_3_072 = _fix(1.961570560), _fix(2.053119869), _fix(
 
 
 def _split_intervals(seg: bytes):
-    """Remove byte stuffing and split at restart markers -> (list of data byte strings, list of RST numbers)."""
+    """Remove byte stuffing and split at restart markers -> (list of data byte strings, list of RST numbers).
+    A marker may be preceded by any number of 0xFF fill bytes (T.81 B.1.1.2); fill bytes that run to the end of
+    the segment precede its EOI."""
     out, marks, cur, i, n = [], [], bytearray(), 0, len(seg)
     while i < n:
         x = seg[i]
@@ -34,17 +36,20 @@ def _split_intervals(seg: bytes):
             cur.append(x)
             i += 1
             continue
-        if i + 1 >= n:
-            raise JpegError("entropy-coded data ends inside a marker")
-        y = seg[i + 1]
-        if y == 0:
+        if i + 1 < n and seg[i + 1] == 0:
             cur.append(0xFF)
-        elif 0xD0 <= y <= 0xD7:
-            out.append(bytes(cur))
-            marks.append(y - 0xD0)
-            cur = bytearray()
-        else:
+            i += 2
+            continue
+        while i + 1 < n and seg[i + 1] == 0xFF:
+            i += 1
+        if i + 1 >= n:
+            break
+        y = seg[i + 1]
+        if not 0xD0 <= y <= 0xD7:
             raise JpegError(f"unexpected marker 0xFF{y:02X} inside the entropy-coded data")
+        out.append(bytes(cur))
+        marks.append(y - 0xD0)
+        cur = bytearray()
         i += 2
     out.append(bytes(cur))
     return out, marks
@@ -59,6 +64,8 @@ def coefficients(buf, info: JpegInfo = None):
     intervals, marks = _split_intervals(seg)
     total = info.mcus_x * info.mcus_y
     per = info.restart if info.restart else total
+    if info.restart and total % per == 0 and len(intervals) == total // per + 1 and not intervals[-1]:
+        intervals.pop()     # an RST after the last MCU, which some encoders write when the last interval is whole
     if len(intervals) != -(-total // per):
         raise JpegError(f"{len(intervals) - 1} restart markers where {-(-total // per) - 1} were expected")
     if any(m != k % 8 for k, m in enumerate(marks)):
