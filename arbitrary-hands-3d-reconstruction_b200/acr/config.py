@@ -48,6 +48,8 @@ _DEFAULTS = dict(
     cam_trans_mode="lstsq",                                # 'lstsq' (device least squares, SURVEY 8f-1) | 'pnp' (device
                                                           # RANSAC-EPnP, the reference's cv2.solvePnPRansac) | 'none'
     return_maps=True,                                      # materialise NCHW fp32 maps lazily on access
+    return_part_labels=False,                              # outputs['part_labels']: per-image uint8 part labels at the
+                                                          # frame's resolution (acr_b200.ops.part_labels, DESIGN.md)
     demo_mode="image", inputs=None, output_dir=None, save_dict_results=False,
 )
 

@@ -46,6 +46,20 @@ def _load_streams(static, stream_ids, stream_begin):
         sbeg.copy_(torch.as_tensor(stream_begin), non_blocking=True)
 
 
+def _label_buffer(part_labels, batch, dev, default_capacity):
+    """The PartLabels of a captured graph: ``part_labels`` None / False = no labels, True = the default capacity, an
+    int = that capacity in label bytes (pixels)."""
+    if part_labels is None or part_labels is False:
+        return None
+    if part_labels is True:
+        if default_capacity is None:
+            raise ValueError("capture_graph(part_labels=...) takes the label capacity in pixels (the frames' "
+                             "H*W summed over the batch), not True")
+        part_labels = default_capacity
+    from acr_b200 import ops as _ops
+    return _ops.PartLabels(int(part_labels), batch, dev)
+
+
 def _device_ints(v, B, dev, name):
     if v is None:
         return None
@@ -173,7 +187,7 @@ class ACR(nn.Module):
 
     @torch.no_grad()
     def fused_forward(self, images_rgb_u8, offsets, out=None, peers=None, tracker=None, stream_ids=None,
-                      stream_begin=None):
+                      stream_begin=None, part_labels=None):
         """Sync-free pipeline: backbone + heads + parse + MANO enqueued back to back; MANO runs over
         the worst case 2KB rows (K = ``max_hands_per_side``) and skips rows >= L+R on the device.  Returns dense
         buffers (zero copy: the parse buffers are shared per batch size, consume them before the next call).  ``peers``
@@ -182,7 +196,11 @@ class ACR(nn.Module):
         stream, tracked (and, with the tracker's smooth_coeff, filtered per track) between parse and MANO;
         mano['track_id'] is the tracker's id buffer.  With a multi-stream tracker (``streams`` > 1), ``stream_ids``
         (B,) int gives each image's stream slot (the frames of one stream in batch order) and ``stream_begin`` (B,)
-        starts a slot over at each nonzero frame; a row's stream is ``stream_ids[reorganize_idx]``."""
+        starts a slot over at each nonzero frame; a row's stream is ``stream_ids[reorganize_idx]``.  ``part_labels``
+        (acr_b200.ops.PartLabels): each image's uint8 part labels at its frame's resolution (``offsets``) are written
+        into that buffer, mano['part_labels'] is the buffer (zero copy, like the parse buffers: consume or copy the
+        labels before the next call into the same buffer).  Host offsets are checked against its capacity before
+        anything is enqueued; device offsets on the device (a frame that does not fit is flagged, not written)."""
         if tracker is not None and peers is not None:
             raise ValueError("a tracker follows one stream: it cannot be combined with a cross-rank vertex gather")
         if tracker is None and (stream_ids is not None or stream_begin is not None):
@@ -194,8 +212,15 @@ class ACR(nn.Module):
         if tracker is not None and tracker.streams > 1 and sid is None:
             raise ValueError(f"this tracker follows {tracker.streams} streams: give stream_ids, the slot of each frame")
         meta = {'image': images_rgb_u8, 'offsets': offsets, 'batch_ids': None}
-        eng, bufs = self.model.forward_dense(meta)
         from acr_b200 import ops as _ops
+        if part_labels is not None and offsets is not None and not torch.as_tensor(offsets).is_cuda:
+            part_labels.expect(torch.as_tensor(offsets, dtype=torch.float32).numpy())
+        eng, bufs = self.model.forward_dense(meta)
+        if part_labels is not None:
+            if offsets is None:
+                S = float(args().input_size)
+                offsets = torch.tensor([[S, S, 0, 0, 0, 0, 0, 0, 0, 0]]).repeat(B, 1)
+            _ops.part_labels(eng.view('segms'), offsets, part_labels)
         ids = _ops.track_hands(bufs, tracker, sid, sbeg) if tracker is not None else None
         ml, mr = self.mano_regression.models()
         mano = _ops.mano_forward(ml, mr, bufs.poses, bufs.betas, bufs.hand_type, 1, self.mano_regression.center_idx,
@@ -205,10 +230,12 @@ class ACR(nn.Module):
                                                     args().focal_length, 512.0, n_dev=bufs.counts[2:3])
         if ids is not None:
             mano['track_id'] = ids
+        if part_labels is not None:
+            mano['part_labels'] = part_labels
         return bufs, mano
 
     @torch.no_grad()
-    def capture_graph(self, batch: int, device=None, tracker=None):
+    def capture_graph(self, batch: int, device=None, tracker=None, part_labels=None):
         """CUDA-graph the whole sync-free pipeline (backbone + heads + parse + MANO + cam_trans, ~380 kernel
         launches) for a fixed batch size: returns ``replay(frames_u8, offsets) -> (bufs, mano)`` that copies
         the inputs into static buffers and launches ONE graph.  This is what makes the reference's
@@ -217,18 +244,22 @@ class ACR(nn.Module):
         (``replay.hands_per_side``); a replay under another value raises.  With a ``tracker`` the graph also tracks:
         each replay continues the tracker's state from the previous one (``tracker.reset()`` starts over).  With a
         multi-stream tracker the replay is ``replay(frames_u8, offsets, stream_ids, stream_begin=None)``: (B,) stream
-        slots and start-over flags per frame, copied into static buffers of the graph."""
+        slots and start-over flags per frame, copied into static buffers of the graph.  ``part_labels`` = a capacity in
+        pixels (the most H*W summed over a replay's frames): the graph also writes each image's part labels into
+        ``replay.part_labels`` (acr_b200.ops.PartLabels), which is mano['part_labels'].  A replay with host offsets
+        that need more raises before anything is enqueued; with device offsets the device flags such frames."""
         from acr.result_parser import ResultParser
         K = ResultParser.hands_per_side()
         _check_tracker(tracker, K)
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         frames = torch.zeros(batch, args().input_size, args().input_size, 3, dtype=torch.uint8, device=dev)
         offsets = torch.zeros(batch, 10, device=dev)
+        labels = _label_buffer(part_labels, batch, dev, None)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
             for _ in range(2):
-                self.fused_forward(frames, offsets)         # (without the tracker: its state stays as it is)
+                self.fused_forward(frames, offsets, part_labels=labels)   # (without the tracker: its state stays)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         streams = _stream_buffers(tracker, batch, dev)
@@ -239,10 +270,17 @@ class ACR(nn.Module):
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             bufs, mano = self.fused_forward(frames, offsets, tracker=tracker, stream_ids=streams and streams[0],
-                                            stream_begin=streams and streams[1])
+                                            stream_begin=streams and streams[1], part_labels=labels)
+
+        def load_labels(offs):
+            if labels is None:
+                return
+            offs = torch.as_tensor(offs)
+            labels.expect(None if offs.is_cuda else offs.to(torch.float32).reshape(batch, 10).numpy())
 
         def replay_one(frames_u8, offs):
             _check_hands_per_side(K)
+            load_labels(offs)
             frames.copy_(frames_u8, non_blocking=True)
             offsets.copy_(offs, non_blocking=True)
             graph.replay()
@@ -250,6 +288,7 @@ class ACR(nn.Module):
 
         def replay_streams(frames_u8, offs, stream_ids=None, stream_begin=None):
             _check_hands_per_side(K)
+            load_labels(offs)
             _load_streams(streams, stream_ids, stream_begin)
             frames.copy_(frames_u8, non_blocking=True)
             offsets.copy_(offs, non_blocking=True)
@@ -258,32 +297,36 @@ class ACR(nn.Module):
 
         replay = replay_one if streams is None else replay_streams
         replay.graph, replay.static_inputs, replay.hands_per_side = graph, (frames, offsets), K
-        replay.static_streams = streams
+        replay.static_streams, replay.part_labels = streams, labels
         return replay
 
     @torch.no_grad()
-    def capture_frames_graph(self, batch: int, max_frame_bytes: int, device=None, tracker=None):
+    def capture_frames_graph(self, batch: int, max_frame_bytes: int, device=None, tracker=None, part_labels=None):
         """``capture_graph`` from raw frames: one CUDA graph of the ragged pre-processing (cubic tables, BGR->RGB,
         white pad, bicubic resize, offsets; acr_b200.preprocess.RaggedFrames) followed by ``fused_forward``.  Returns
         ``replay(frames) -> (bufs, mano)`` for a list of exactly ``batch`` BGR frames (numpy arrays, CPU or CUDA
         tensors) of any sizes, each replay its own, whose packed H*W*3 bytes sum to at most ``max_frame_bytes``.  Host
         frames travel in one H2D copy; a list that does not fit raises before anything is enqueued.  Like
         ``capture_graph``, the graph is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with
-        a multi-stream tracker the replay is ``replay(frames, stream_ids, stream_begin=None)``."""
+        a multi-stream tracker the replay is ``replay(frames, stream_ids, stream_begin=None)``.  ``part_labels`` True (a
+        capacity of ``max_frame_bytes // 3`` pixels, which every replay fits) or a capacity in pixels: the graph also
+        writes each frame's part labels into ``replay.part_labels`` (acr_b200.ops.PartLabels, mano['part_labels']);
+        ``replay.part_labels[i]`` is frame i's (H_i, W_i) view."""
         from acr.result_parser import ResultParser
-        from acr_b200.preprocess import RaggedFrames
+        from acr_b200.preprocess import RaggedFrames, ragged_layout
         K = ResultParser.hands_per_side()
         _check_tracker(tracker, K)
         import numpy as np
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
+        labels = _label_buffer(part_labels, batch, dev, max_frame_bytes // 3)
         cur = torch.cuda.current_stream(dev)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(cur)
         with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
             rf.load([np.full((1, 1, 3), 255, np.uint8)] * batch)
             for _ in range(2):
-                self.fused_forward(*rf.launch())
+                self.fused_forward(*rf.launch(), part_labels=labels)
         cur.wait_stream(side)
         torch.cuda.synchronize(dev)
         streams = _stream_buffers(tracker, batch, dev)
@@ -294,10 +337,15 @@ class ACR(nn.Module):
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker, stream_ids=streams and streams[0],
-                                            stream_begin=streams and streams[1])
+                                            stream_begin=streams and streams[1], part_labels=labels)
+
+        def load_labels(frames):
+            if labels is not None:
+                labels.expect(ragged_layout(frames)[1])
 
         def replay_one(frames):
             _check_hands_per_side(K)
+            load_labels(frames)
             rf.load(frames)
             graph.replay()
             return bufs, mano
@@ -306,6 +354,7 @@ class ACR(nn.Module):
             _check_hands_per_side(K)
             if len(frames) != batch:                        # RaggedFrames checks it too, but after the stream ids
                 raise ValueError(f"this graph takes exactly {batch} frames, got {len(frames)}")
+            load_labels(frames)
             _load_streams(streams, stream_ids, stream_begin)
             rf.load(frames)
             graph.replay()
@@ -313,12 +362,12 @@ class ACR(nn.Module):
 
         replay = replay_one if streams is None else replay_streams
         replay.graph, replay.frames, replay.hands_per_side = graph, rf, K
-        replay.static_streams = streams
+        replay.static_streams, replay.part_labels = streams, labels
         return replay
 
     @torch.no_grad()
     def capture_jpeg_graph(self, batch: int, max_coded_bytes: int, max_frame_bytes: int, tracker=None, device=None,
-                           max_blocks: int = None):
+                           max_blocks: int = None, part_labels=None):
         """``capture_frames_graph`` from JPEG files: one CUDA graph of the device JPEG decode (acr_b200.jpeg), the
         ragged pre-processing and ``fused_forward``.  Returns ``replay(encoded_list) -> (bufs, mano)`` for exactly
         ``batch`` baseline JPEG files (bytes-like) whose entropy-coded bytes sum to at most ``max_coded_bytes`` and
@@ -330,10 +379,11 @@ class ACR(nn.Module):
         work past each file's size.  Corrupt entropy-coded data sets the per-file status words and gives that frame
         an all-black image; ``replay.jpeg.raise_on_status()`` waits and raises.  Like ``capture_graph``, the graph
         is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with a multi-stream tracker the replay is
-        ``replay(encoded_list, stream_ids, stream_begin=None)``."""
+        ``replay(encoded_list, stream_ids, stream_begin=None)``.  ``part_labels`` as in ``capture_frames_graph``: True
+        (``max_frame_bytes // 3`` pixels) or a capacity, the labels in ``replay.part_labels``."""
         from acr.result_parser import ResultParser
         from acr_b200 import jpeg
-        from acr_b200.preprocess import RaggedFrames
+        from acr_b200.preprocess import RaggedFrames, shapes_layout
         import cv2
         import numpy as np
         K = ResultParser.hands_per_side()
@@ -345,9 +395,12 @@ class ACR(nn.Module):
         jb = jpeg.JpegBatch(batch, max_coded_bytes, max_frame_bytes, -(-max_coded_bytes // jpeg.CHUNK) + batch,
                             max_blocks, dev, out=rf.packed)
         warm = [cv2.imencode(".jpg", np.full((1, 1, 3), 255, np.uint8))[1].tobytes()] * batch
+        labels = _label_buffer(part_labels, batch, dev, max_frame_bytes // 3)
 
         def load(encoded, lay):
             shapes = [(int(d["H"]), int(d["W"])) for d in lay.desc]
+            if labels is not None:
+                labels.expect(shapes_layout(shapes)[1])
             rf.load_shapes(shapes)
             jb.load(encoded, lay)
 
@@ -358,7 +411,7 @@ class ACR(nn.Module):
             load(warm, jb.prepare(warm, exact=True)[0])
             for _ in range(2):
                 jb.launch(batch)
-                self.fused_forward(*rf.launch())
+                self.fused_forward(*rf.launch(), part_labels=labels)
         cur.wait_stream(side)
         torch.cuda.synchronize(dev)
         streams = _stream_buffers(tracker, batch, dev)
@@ -370,7 +423,7 @@ class ACR(nn.Module):
         with torch.cuda.graph(graph):
             jb.launch(batch)
             bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker, stream_ids=streams and streams[0],
-                                            stream_begin=streams and streams[1])
+                                            stream_begin=streams and streams[1], part_labels=labels)
 
         def replay_one(encoded_list):
             _check_hands_per_side(K)
@@ -390,7 +443,7 @@ class ACR(nn.Module):
 
         replay = replay_one if streams is None else replay_streams
         replay.graph, replay.frames, replay.jpeg, replay.hands_per_side = graph, rf, jb, K
-        replay.static_streams = streams
+        replay.static_streams, replay.part_labels = streams, labels
         return replay
 
     @torch.no_grad()

@@ -179,11 +179,27 @@ class ACR(nn.Module):
         img, dev = self._image(meta_data)
         eng = self.engine(img.shape[0], dev)
         eng.run(img)
+        labels = self._part_labels(eng, meta_data) if args().return_part_labels else None
         outputs = LazyOutputs(eng if args().return_maps else None)
+        if labels is not None:
+            outputs['part_labels'] = labels.views()
         bufs = self._result_parser.launch(eng.parse_inputs(), img.shape[0], meta_data, dev)
         outputs, meta_data = self._result_parser.collect(bufs, outputs, meta_data)
         outputs['meta_data'] = meta_data
         return outputs
+
+    def _part_labels(self, eng, meta_data):
+        """``return_part_labels``: enqueue the labels of this run's ``segms`` into a fresh buffer sized for the frames
+        of meta_data['offsets'] (the input square when there are none), before the next run can reuse the arena."""
+        from acr_b200 import ops as _ops
+        offs = meta_data.get('offsets')
+        if offs is None:
+            S = float(args().input_size)
+            offs = torch.tensor([[S, S, 0, 0, 0, 0, 0, 0, 0, 0]]).repeat(eng.batch, 1)
+        offs = torch.as_tensor(offs).detach().to('cpu', torch.float32)
+        total = _ops.part_label_layout(offs.numpy(), 0)[2]
+        buf = _ops.PartLabels(total, eng.batch, eng.device)
+        return _ops.part_labels(eng.view('segms'), offs, buf)
 
     @torch.no_grad()
     def forward_dense(self, meta_data):

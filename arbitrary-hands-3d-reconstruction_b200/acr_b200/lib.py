@@ -71,7 +71,7 @@ _lib: Optional[C.CDLL] = None
 EXPORTS = ["acr_b200_last_error", "acr_b200_version", "acr_b200_mano_model_floats", "acr_b200_mano_pack_model",
            "acr_b200_mano_forward", "acr_b200_mano_forward_gather", "acr_b200_gather_wait",
            "acr_b200_mano_backward_workspace_floats", "acr_b200_mano_backward", "acr_b200_mano_layer_forward",
-           "acr_b200_mano_layer_backward", "acr_b200_mano_layer_jvp", "acr_b200_cam_trans", "acr_b200_cam_trans_pnp", "acr_b200_preprocess", "acr_b200_cubic_tables", "acr_b200_preprocess_ragged", "acr_b200_track_state_bytes", "acr_b200_track_hands", "acr_b200_track_streams_workspace_bytes", "acr_b200_track_streams", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse", "acr_b200_parse_topk",
+           "acr_b200_mano_layer_backward", "acr_b200_mano_layer_jvp", "acr_b200_cam_trans", "acr_b200_cam_trans_pnp", "acr_b200_preprocess", "acr_b200_cubic_tables", "acr_b200_preprocess_ragged", "acr_b200_part_labels", "acr_b200_track_state_bytes", "acr_b200_track_hands", "acr_b200_track_streams_workspace_bytes", "acr_b200_track_streams", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse", "acr_b200_parse_topk",
            "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_profile_ops", "acr_b200_plan_num_launches", "acr_b200_plan_op_launch", "acr_b200_plan_destroy",
            "acr_b200_run_op", "acr_b200_pack_conv", "acr_b200_jpeg_workspace_bytes", "acr_b200_jpeg_coef_offset", "acr_b200_jpeg_decode"]
 
@@ -105,6 +105,7 @@ def load() -> C.CDLL:
     lib.acr_b200_preprocess.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, i32, i32, i32, i32, vp, vp]
     lib.acr_b200_cubic_tables.argtypes = [vp, i32, i32, vp, vp, vp]
     lib.acr_b200_preprocess_ragged.argtypes = [vp, C.c_int64, vp, i32, vp, vp, i32, vp, vp, vp]
+    lib.acr_b200_part_labels.argtypes = [vp, i32, i32, i32, vp, i32, C.c_int64, vp, vp, vp, vp]
     lib.acr_b200_track_state_bytes.argtypes = [i32]
     lib.acr_b200_track_state_bytes.restype = C.c_size_t
     lib.acr_b200_track_hands.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp]

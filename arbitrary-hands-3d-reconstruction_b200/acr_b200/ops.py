@@ -422,3 +422,123 @@ def parse_maps(maps: Dict[str, tuple], B: int, bufs: ParseBuffers, meta_batch_id
     L.check(rc, "parse")
     # keep the inputs alive until the kernels have run
     bufs._keep = (meta_batch_ids, offsets, [m for m in maps.values()])
+
+
+# --------------------------------------------------------------------------------- part labels
+PART_LABELS_MAX_SIDE = 16384                       # ACR_B200_PART_LABELS_MAX_SIDE
+PART_LABELS_INVALID, PART_LABELS_OVER_CAPACITY = 1, 2   # ACR_B200_PART_LABELS_* flags
+PART_LABEL_CLASSES = 33                           # 0 background, 1-16 right-hand parts, 17-32 left-hand parts
+
+
+def part_label_geometry(offsets) -> np.ndarray:
+    """The packing rule of acr_b200_part_labels on the host: (n,10) offsets rows -> (n,3) int64 [first label byte, H,
+    W], (0, 0) for an invalid row (which then takes no bytes).  ``part_label_layout`` adds the flags."""
+    o = np.asarray(offsets, np.float32).reshape(-1, 10)
+    ok = np.all((o >= 0) & (o == np.floor(o)), axis=1) & (o[:, 0] == o[:, 1]) & (o[:, 0] >= 1) \
+        & (o[:, 0] <= PART_LABELS_MAX_SIDE) & (o[:, 6] + o[:, 8] < o[:, 0]) & (o[:, 7] + o[:, 9] < o[:, 0])
+    geo = np.zeros((len(o), 3), np.int64)
+    with np.errstate(invalid="ignore"):
+        geo[ok, 1] = (o[ok, 0] - o[ok, 6] - o[ok, 8]).astype(np.int64)
+        geo[ok, 2] = (o[ok, 0] - o[ok, 7] - o[ok, 9]).astype(np.int64)
+    sizes = geo[:, 1] * geo[:, 2]
+    geo[:, 0] = np.cumsum(sizes) - sizes
+    return geo
+
+
+def part_label_layout(offsets, capacity: int):
+    """-> (geometry (n,3) as ``part_label_geometry``, flags (n,) int32, total label bytes of the valid frames): what
+    acr_b200_part_labels computes on the device for these offsets and this capacity."""
+    geo = part_label_geometry(offsets)
+    valid = geo[:, 1] > 0
+    flags = np.where(valid, 0, PART_LABELS_INVALID).astype(np.int32)
+    flags[valid & (geo[:, 0] + geo[:, 1] * geo[:, 2] > capacity)] = PART_LABELS_OVER_CAPACITY
+    return geo, flags, int((geo[:, 1] * geo[:, 2]).sum())
+
+
+class PartLabels:
+    """Output buffer of ``part_labels``: ``capacity`` label bytes and per-frame offsets / flags for up to
+    ``max_frames`` images, allocated once and written in place (zero copy, like ParseBuffers: a later launch into the
+    same buffer overwrites the labels, so consume or copy them first).  ``labels[i]`` is image i's (H_i, W_i) uint8
+    CUDA view (0 background, 1-16 right-hand parts, 17-32 left-hand parts); a frame flagged invalid or over capacity
+    raises.  When the launch had its offsets on the host the views need no device read; otherwise the first index
+    reads the offsets and flags back (one synchronisation)."""
+
+    def __init__(self, capacity: int, max_frames: int, device=None):
+        if int(capacity) < 0 or int(max_frames) < 1:
+            raise ValueError(f"PartLabels: need capacity >= 0 and max_frames >= 1 (got {capacity}, {max_frames})")
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.capacity, self.max_frames = int(capacity), int(max_frames)
+        self.data = torch.empty(max(self.capacity, 1), dtype=torch.uint8, device=self.device)
+        self.frame_offset = torch.zeros(self.max_frames, dtype=torch.int64, device=self.device)
+        self.flags = torch.zeros(self.max_frames, dtype=torch.int32, device=self.device)
+        self.n = 0
+        self._host = None        # (geometry, flags) of the last launch when its offsets were on the host
+        self._offsets = None     # the device offsets of the last launch
+
+    def __len__(self) -> int:
+        return self.n
+
+    def expect(self, offsets) -> None:
+        """Check the frames of the next launch, (n,10) host offsets rows, against the capacity (ValueError before
+        anything is enqueued) and keep their geometry for the views; None forgets it (device offsets: the views read
+        the launch's offsets back)."""
+        if offsets is None:
+            self._host = None
+            return
+        geo, flags, total = part_label_layout(offsets, self.capacity)
+        if (flags == PART_LABELS_OVER_CAPACITY).any():
+            raise ValueError(f"part_labels: the frames need {total} label bytes, over the capacity of {self.capacity}")
+        self._host = (geo, flags)
+
+    def _layout(self):
+        if self._host is None:
+            self._host = part_label_layout(self._offsets[:self.n].cpu().numpy(), self.capacity)[:2]
+        return self._host
+
+    def __getitem__(self, i: int) -> torch.Tensor:
+        if not -self.n <= i < self.n:
+            raise IndexError(f"image {i} of {self.n}")
+        i %= self.n
+        geo, flags = self._layout()
+        if flags[i]:
+            why = "its offsets row is not a valid geometry" if flags[i] == PART_LABELS_INVALID else \
+                f"its labels end past the capacity of {self.capacity} bytes"
+            raise ValueError(f"image {i} has no part labels: {why}")
+        o, H, W = (int(v) for v in geo[i])
+        return self.data[o:o + H * W].view(H, W)
+
+    def views(self):
+        """Every image's (H, W) view, in batch order."""
+        return [self[i] for i in range(self.n)]
+
+
+def part_labels(segms: torch.Tensor, offsets, out: PartLabels) -> PartLabels:
+    """Enqueue acr_b200_part_labels on the current stream: ``segms`` the (n, M, M, stride) NHWC logit map as it lies in
+    the arena (Engine.view('segms'): bf16 / fp16 / fp32, stride 48), ``offsets`` (n,10) the frames' offsets rows, on
+    the host or the device.  Host offsets are checked against ``out``'s capacity before anything is enqueued
+    (ValueError); device offsets are checked on the device, which flags what does not fit.  Returns ``out``."""
+    n = int(segms.shape[0])
+    dt = {torch.bfloat16: L.DT_BF16, torch.float16: L.DT_F16, torch.float32: L.DT_F32}.get(segms.dtype)
+    if dt is None or segms.dim() != 4 or segms.shape[1] != segms.shape[2] or segms.stride(3) != 1 \
+            or segms.stride(2) * segms.shape[2] != segms.stride(1) or segms.stride(1) * segms.shape[1] != segms.stride(0):
+        raise ValueError("part_labels: segms must be an (n, M, M, stride) NHWC bf16 / fp16 / fp32 map with "
+                         "contiguous rows")
+    if n > out.max_frames:
+        raise ValueError(f"part_labels: {n} images exceed the buffer's {out.max_frames} frames")
+    offsets = torch.as_tensor(offsets)
+    if tuple(offsets.shape) != (n, 10):
+        raise ValueError(f"part_labels: offsets must have shape ({n}, 10), got {tuple(offsets.shape)}")
+    host = None
+    if not offsets.is_cuda:
+        host = offsets.to(torch.float32).numpy()
+        out.expect(host)
+    dev = L.require_cuda(segms, out.data)
+    offs_dev = offsets.to(device=dev, dtype=torch.float32).contiguous()
+    with L.on(dev):
+        L.check(L.load().acr_b200_part_labels(L.ptr(segms), dt, int(segms.stride(2)), int(segms.shape[1]),
+                                              L.ptr(offs_dev), n, out.capacity, L.ptr(out.data),
+                                              L.ptr(out.frame_offset), L.ptr(out.flags), L.current_stream(dev)),
+                "part_labels")
+    out.n, out._offsets = n, offs_dev
+    out._host = None if host is None else part_label_layout(host, out.capacity)[:2]
+    return out

@@ -226,6 +226,29 @@ int acr_b200_preprocess_ragged(const uint8_t* frames_bgr, int64_t src_bytes, con
                                const int16_t* coef, const int32_t* ofs, int out_size, uint8_t* out_rgb,
                                float* offsets, void* stream);
 
+/* Part labels: SegmNet's 33-class logits -> one uint8 label per pixel of each frame (0 background, 1-16 right-hand
+ * parts, 17-32 left-hand parts; the network's channel order).  segms: n maps of map_size x map_size pixels, NHWC with
+ * pix_stride elements per pixel (the arena's `segms`: 48), dtype ACR_DT_BF16 / ACR_DT_F16 / ACR_DT_F32, channels
+ * 0..32 the logits, 16-byte aligned.  offsets (n,10) fp32 on the device: image i's row [side, side, 0,0,0,0, pad_t,
+ * pad_r, pad_b, pad_l] (the pj2d_org offsets) gives its frame of H = side - pad_t - pad_b rows and W = side - pad_l -
+ * pad_r columns, and
+ *   labels_i[y, x] = argmax_c bilinear(segms_i[c], side)[y + pad_t, x + pad_l]
+ * with F.interpolate(size=(side, side), mode='bilinear', align_corners=False) weights, interpolated in fp32, ties to
+ * the lowest channel (tests/part_labels_ref.py is the statement).  Frame i's H*W bytes start frame_offset[i] bytes
+ * into `labels`: the exclusive prefix of H*W over the frames before it (a flagged frame counts 0 when its geometry is
+ * invalid).  flags[i] (int32): ACR_B200_PART_LABELS_INVALID when the row has a negative or non-integer entry, unequal
+ * sides, a side outside 1..ACR_B200_PART_LABELS_MAX_SIDE, pad_t + pad_b >= side or pad_l + pad_r >= side;
+ * ACR_B200_PART_LABELS_OVER_CAPACITY when its labels would end past `capacity` bytes; 0 otherwise.  A flagged frame
+ * gets no stores.  The geometry is read on the device and the grids depend on n and map_size only, so a graph replay
+ * may change every frame's size.  Two launches (the prefix, then one CTA per 16 x 16 source quads and image); no
+ * atomics, the same bytes on every call.  A NULL argument, another dtype, a stride that does not cover 33 channels in
+ * 16-byte loads, n outside 1..65535, map_size outside 1..4096 or capacity < 0 is ACR_B200_EINVAL.                  */
+#define ACR_B200_PART_LABELS_MAX_SIDE 16384
+#define ACR_B200_PART_LABELS_INVALID 1
+#define ACR_B200_PART_LABELS_OVER_CAPACITY 2
+int acr_b200_part_labels(const void* segms, int dtype, int pix_stride, int map_size, const float* offsets, int n,
+                         int64_t capacity, uint8_t* labels, int64_t* frame_offset, int32_t* flags, void* stream);
+
 /* Multi-hand tracking of one stream between parse and MANO: a stable track id per detected hand and one OneEuro
  * bank per track, for up to K hands per side (the parse's max_hands_per_side).  The filter replaces OneEuroFilter /
  * LowPassFilter (acr/utils.py:1485-1527), smooth_results (:1478-1482), smooth_global_rot_matrix (:1466-1470) and the
