@@ -2,6 +2,9 @@
 hot path only: model -> parse -> MANO.  Rendering / visualisation / CLI loops are out of scope."""
 from __future__ import annotations
 
+import inspect
+from typing import Callable, NamedTuple
+
 import torch
 import torch.nn as nn
 
@@ -31,19 +34,37 @@ def _stream_buffers(tracker, batch, dev):
     return (torch.zeros(batch, dtype=torch.int32, device=dev), torch.zeros(batch, dtype=torch.int32, device=dev))
 
 
-def _load_streams(static, stream_ids, stream_begin):
-    """Check a replay's stream ids / begin flags (before anything is enqueued), then copy them into the graph's."""
-    sid, sbeg = static
-    for name, v in (("stream_ids", stream_ids), ("stream_begin", stream_begin)):
-        if v is not None and tuple(torch.as_tensor(v).shape) != tuple(sid.shape):
-            raise ValueError(f"{name} must have shape {tuple(sid.shape)}, got {tuple(torch.as_tensor(v).shape)}")
-    if stream_ids is None:
+def _check_streams(static, stream_ids, stream_begin):
+    """A replay's stream ids / begin flags as tensors (stream_begin may stay None), checked against the graph's."""
+    shape = tuple(static[0].shape)
+    ids, begin = (None if v is None else torch.as_tensor(v) for v in (stream_ids, stream_begin))
+    for name, t in (("stream_ids", ids), ("stream_begin", begin)):
+        if t is not None and tuple(t.shape) != shape:
+            raise ValueError(f"{name} must have shape {shape}, got {tuple(t.shape)}")
+    if ids is None:
         raise ValueError("this graph tracks several streams: replay needs stream_ids, the stream slot of each frame")
-    sid.copy_(torch.as_tensor(stream_ids), non_blocking=True)
-    if stream_begin is None:
-        sbeg.zero_()
-    else:
-        sbeg.copy_(torch.as_tensor(stream_begin), non_blocking=True)
+    return ids, begin
+
+
+def _check_copy(name, src, dst):
+    """Raise unless ``dst.copy_(src)`` takes ``src``: a tensor whose shape broadcasts to ``dst``'s."""
+    if not isinstance(src, torch.Tensor):
+        raise TypeError(f"{name} must be a tensor, got {type(src).__name__}")
+    if src.shape != dst.shape and (src.dim() > dst.dim() or
+                                   any(s not in (1, d) for s, d in zip(reversed(src.shape), reversed(dst.shape)))):
+        raise ValueError(f"{name} of shape {tuple(src.shape)} does not broadcast to the graph's {tuple(dst.shape)}")
+
+
+class _InputStage(NamedTuple):
+    """How a captured graph gets its frames.  ``check(*inputs)`` runs every check of a replay's inputs and writes
+    nothing -> (what ``load`` takes, the frames' (B,10) host offsets rows for the part labels, or None when the
+    offsets are on the device or the graph has no labels);
+    ``load`` copies them into the graph's buffers; ``enqueue()`` launches the input kernels -> (frames, offsets) on the
+    device, as ``fused_forward`` takes them; ``attrs`` are the replay's attributes of this input."""
+    check: Callable
+    load: Callable
+    enqueue: Callable
+    attrs: dict
 
 
 def _label_buffer(part_labels, batch, dev, default_capacity):
@@ -248,57 +269,23 @@ class ACR(nn.Module):
         pixels (the most H*W summed over a replay's frames): the graph also writes each image's part labels into
         ``replay.part_labels`` (acr_b200.ops.PartLabels), which is mano['part_labels'].  A replay with host offsets
         that need more raises before anything is enqueued; with device offsets the device flags such frames."""
-        from acr.result_parser import ResultParser
-        K = ResultParser.hands_per_side()
-        _check_tracker(tracker, K)
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         frames = torch.zeros(batch, args().input_size, args().input_size, 3, dtype=torch.uint8, device=dev)
         offsets = torch.zeros(batch, 10, device=dev)
         labels = _label_buffer(part_labels, batch, dev, None)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
-            for _ in range(2):
-                self.fused_forward(frames, offsets, part_labels=labels)   # (without the tracker: its state stays)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
-        streams = _stream_buffers(tracker, batch, dev)
-        if tracker is not None:
-            tracker.ids(batch)                              # the id buffer exists before the capture
-            if streams is not None:
-                tracker.workspace(batch)                    # and the workspace
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            bufs, mano = self.fused_forward(frames, offsets, tracker=tracker, stream_ids=streams and streams[0],
-                                            stream_begin=streams and streams[1], part_labels=labels)
 
-        def load_labels(offs):
-            if labels is None:
-                return
-            offs = torch.as_tensor(offs)
-            labels.expect(None if offs.is_cuda else offs.to(torch.float32).reshape(batch, 10).numpy())
+        def check(frames_u8, offs):
+            _check_copy("frames", frames_u8, frames)
+            _check_copy("offsets", offs, offsets)
+            host = labels is not None and not offs.is_cuda
+            return (frames_u8, offs), offs.to(torch.float32).expand(batch, 10).numpy() if host else None
 
-        def replay_one(frames_u8, offs):
-            _check_hands_per_side(K)
-            load_labels(offs)
-            frames.copy_(frames_u8, non_blocking=True)
-            offsets.copy_(offs, non_blocking=True)
-            graph.replay()
-            return bufs, mano
+        def load(inputs):
+            frames.copy_(inputs[0], non_blocking=True)
+            offsets.copy_(inputs[1], non_blocking=True)
 
-        def replay_streams(frames_u8, offs, stream_ids=None, stream_begin=None):
-            _check_hands_per_side(K)
-            load_labels(offs)
-            _load_streams(streams, stream_ids, stream_begin)
-            frames.copy_(frames_u8, non_blocking=True)
-            offsets.copy_(offs, non_blocking=True)
-            graph.replay()
-            return bufs, mano
-
-        replay = replay_one if streams is None else replay_streams
-        replay.graph, replay.static_inputs, replay.hands_per_side = graph, (frames, offsets), K
-        replay.static_streams, replay.part_labels = streams, labels
-        return replay
+        stage = _InputStage(check, load, lambda: (frames, offsets), {"static_inputs": (frames, offsets)})
+        return self._capture(batch, dev, tracker, labels, stage)
 
     @torch.no_grad()
     def capture_frames_graph(self, batch: int, max_frame_bytes: int, device=None, tracker=None, part_labels=None):
@@ -306,64 +293,19 @@ class ACR(nn.Module):
         white pad, bicubic resize, offsets; acr_b200.preprocess.RaggedFrames) followed by ``fused_forward``.  Returns
         ``replay(frames) -> (bufs, mano)`` for a list of exactly ``batch`` BGR frames (numpy arrays, CPU or CUDA
         tensors) of any sizes, each replay its own, whose packed H*W*3 bytes sum to at most ``max_frame_bytes``.  Host
-        frames travel in one H2D copy; a list that does not fit raises before anything is enqueued.  Like
+        frames travel in one H2D copy; a list that does not fit raises before anything is written.  Like
         ``capture_graph``, the graph is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with
         a multi-stream tracker the replay is ``replay(frames, stream_ids, stream_begin=None)``.  ``part_labels`` True (a
         capacity of ``max_frame_bytes // 3`` pixels, which every replay fits) or a capacity in pixels: the graph also
         writes each frame's part labels into ``replay.part_labels`` (acr_b200.ops.PartLabels, mano['part_labels']);
         ``replay.part_labels[i]`` is frame i's (H_i, W_i) view."""
-        from acr.result_parser import ResultParser
-        from acr_b200.preprocess import RaggedFrames, ragged_layout
-        K = ResultParser.hands_per_side()
-        _check_tracker(tracker, K)
+        from acr_b200.preprocess import RaggedFrames
         import numpy as np
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
         labels = _label_buffer(part_labels, batch, dev, max_frame_bytes // 3)
-        cur = torch.cuda.current_stream(dev)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(cur)
-        with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
-            rf.load([np.full((1, 1, 3), 255, np.uint8)] * batch)
-            for _ in range(2):
-                self.fused_forward(*rf.launch(), part_labels=labels)
-        cur.wait_stream(side)
-        torch.cuda.synchronize(dev)
-        streams = _stream_buffers(tracker, batch, dev)
-        if tracker is not None:
-            tracker.ids(batch)
-            if streams is not None:
-                tracker.workspace(batch)
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker, stream_ids=streams and streams[0],
-                                            stream_begin=streams and streams[1], part_labels=labels)
-
-        def load_labels(frames):
-            if labels is not None:
-                labels.expect(ragged_layout(frames)[1])
-
-        def replay_one(frames):
-            _check_hands_per_side(K)
-            load_labels(frames)
-            rf.load(frames)
-            graph.replay()
-            return bufs, mano
-
-        def replay_streams(frames, stream_ids=None, stream_begin=None):
-            _check_hands_per_side(K)
-            if len(frames) != batch:                        # RaggedFrames checks it too, but after the stream ids
-                raise ValueError(f"this graph takes exactly {batch} frames, got {len(frames)}")
-            load_labels(frames)
-            _load_streams(streams, stream_ids, stream_begin)
-            rf.load(frames)
-            graph.replay()
-            return bufs, mano
-
-        replay = replay_one if streams is None else replay_streams
-        replay.graph, replay.frames, replay.hands_per_side = graph, rf, K
-        replay.static_streams, replay.part_labels = streams, labels
-        return replay
+        stage = _InputStage(lambda frames: (frames, rf.check(frames)[1]), rf.load, rf.launch, {"frames": rf})
+        return self._capture(batch, dev, tracker, labels, stage, warm=[np.full((1, 1, 3), 255, np.uint8)] * batch)
 
     @torch.no_grad()
     def capture_jpeg_graph(self, batch: int, max_coded_bytes: int, max_frame_bytes: int, tracker=None, device=None,
@@ -374,76 +316,101 @@ class ACR(nn.Module):
         whose decoded H*W*3 bytes sum to at most ``max_frame_bytes``; ``max_blocks`` caps the 8x8 coefficient blocks
         (default ``max_frame_bytes // 48 + 64 * batch``: enough for every sampling when each frame is at least 18
         pixels on each side; thin frames pad more per pixel, a 1x1920 frame needs 720 blocks, so give a larger cap).
-        The replay parses the headers and checks the caps and the supported features before anything is enqueued
+        The replay parses the headers and checks the caps and the supported features before anything is written
         (ValueError / acr_b200.jpeg.JpegUnsupported); the decode's grids are sized by the caps and the device skips
         work past each file's size.  Corrupt entropy-coded data sets the per-file status words and gives that frame
         an all-black image; ``replay.jpeg.raise_on_status()`` waits and raises.  Like ``capture_graph``, the graph
         is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with a multi-stream tracker the replay is
         ``replay(encoded_list, stream_ids, stream_begin=None)``.  ``part_labels`` as in ``capture_frames_graph``: True
         (``max_frame_bytes // 3`` pixels) or a capacity, the labels in ``replay.part_labels``."""
-        from acr.result_parser import ResultParser
         from acr_b200 import jpeg
         from acr_b200.preprocess import RaggedFrames, shapes_layout
         import cv2
         import numpy as np
-        K = ResultParser.hands_per_side()
-        _check_tracker(tracker, K)
         dev = torch.device(device) if device is not None else next(self.model.parameters()).device
         if max_blocks is None:
             max_blocks = max_frame_bytes // 48 + 64 * batch
         rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
         jb = jpeg.JpegBatch(batch, max_coded_bytes, max_frame_bytes, -(-max_coded_bytes // jpeg.CHUNK) + batch,
                             max_blocks, dev, out=rf.packed)
-        warm = [cv2.imencode(".jpg", np.full((1, 1, 3), 255, np.uint8))[1].tobytes()] * batch
         labels = _label_buffer(part_labels, batch, dev, max_frame_bytes // 3)
 
-        def load(encoded, lay):
+        def check(encoded_list):
+            encoded_list = list(encoded_list)
+            lay, _ = jb.prepare(encoded_list, exact=True)
             shapes = [(int(d["H"]), int(d["W"])) for d in lay.desc]
-            if labels is not None:
-                labels.expect(shapes_layout(shapes)[1])
-            rf.load_shapes(shapes)
-            jb.load(encoded, lay)
+            return (encoded_list, lay, shapes), None if labels is None else shapes_layout(shapes)[1]
 
-        cur = torch.cuda.current_stream(dev)
+        def load(prepared):
+            encoded_list, lay, shapes = prepared
+            rf.load_shapes(shapes)
+            jb.load(encoded_list, lay)
+
+        def enqueue():
+            jb.launch(batch)
+            return rf.launch()
+
+        warm = [cv2.imencode(".jpg", np.full((1, 1, 3), 255, np.uint8))[1].tobytes()] * batch
+        stage = _InputStage(check, load, enqueue, {"frames": rf, "jpeg": jb})
+        return self._capture(batch, dev, tracker, labels, stage, warm=warm)
+
+    def _capture(self, batch, dev, tracker, labels, stage, warm=None):
+        """The capture methods' graph: ``stage``'s input kernels, then ``fused_forward`` with ``tracker`` and the
+        ``labels`` buffer -> ``replay``, which takes ``stage.check``'s arguments (then ``stream_ids`` and
+        ``stream_begin`` with a multi-stream tracker).  A replay runs every check before it writes anything, so one
+        that raises leaves the graph's inputs as the last replay left them.  ``warm``: the warm-up's input, loaded
+        through the stage (None: the buffers as they are)."""
+        from acr.result_parser import ResultParser
+        K = ResultParser.hands_per_side()
+        _check_tracker(tracker, K)
         side = torch.cuda.Stream(device=dev)
-        side.wait_stream(cur)
+        side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):                       # warm-up: builds the engine, sets func attributes
-            load(warm, jb.prepare(warm, exact=True)[0])
+            if warm is not None:
+                stage.load(stage.check(warm)[0])
             for _ in range(2):
-                jb.launch(batch)
-                self.fused_forward(*rf.launch(), part_labels=labels)
-        cur.wait_stream(side)
+                self.fused_forward(*stage.enqueue(), part_labels=labels)   # (without the tracker: its state stays)
+        torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         streams = _stream_buffers(tracker, batch, dev)
         if tracker is not None:
-            tracker.ids(batch)
+            tracker.ids(batch)                              # the id buffer exists before the capture
             if streams is not None:
-                tracker.workspace(batch)
+                tracker.workspace(batch)                    # and the workspace
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            jb.launch(batch)
-            bufs, mano = self.fused_forward(*rf.launch(), tracker=tracker, stream_ids=streams and streams[0],
+            bufs, mano = self.fused_forward(*stage.enqueue(), tracker=tracker, stream_ids=streams and streams[0],
                                             stream_begin=streams and streams[1], part_labels=labels)
 
-        def replay_one(encoded_list):
+        params = list(inspect.signature(stage.check).parameters.values())
+        if streams is not None:
+            params += [inspect.Parameter(name, inspect.Parameter.POSITIONAL_OR_KEYWORD, default=None)
+                       for name in ("stream_ids", "stream_begin")]
+        signature = inspect.Signature(params)
+
+        def replay(*args, **kwargs):
+            inputs = signature.bind(*args, **kwargs).arguments
+            stream_ids, stream_begin = (inputs.pop(name, None) for name in ("stream_ids", "stream_begin"))
             _check_hands_per_side(K)
-            encoded_list = list(encoded_list)
-            load(encoded_list, jb.prepare(encoded_list, exact=True)[0])
+            prepared, host_offsets = stage.check(**inputs)
+            if streams is not None:
+                stream_ids, stream_begin = _check_streams(streams, stream_ids, stream_begin)
+            if labels is not None:
+                labels.expect(host_offsets)                 # the last check: it keeps the frames' geometry
+            stage.load(prepared)
+            if streams is not None:
+                streams[0].copy_(stream_ids, non_blocking=True)
+                if stream_begin is None:
+                    streams[1].zero_()
+                else:
+                    streams[1].copy_(stream_begin, non_blocking=True)
             graph.replay()
             return bufs, mano
 
-        def replay_streams(encoded_list, stream_ids=None, stream_begin=None):
-            _check_hands_per_side(K)
-            encoded_list = list(encoded_list)
-            lay, _ = jb.prepare(encoded_list, exact=True)   # every check before the stream ids are copied
-            _load_streams(streams, stream_ids, stream_begin)
-            load(encoded_list, lay)
-            graph.replay()
-            return bufs, mano
-
-        replay = replay_one if streams is None else replay_streams
-        replay.graph, replay.frames, replay.jpeg, replay.hands_per_side = graph, rf, jb, K
-        replay.static_streams, replay.part_labels = streams, labels
+        replay.__signature__ = signature
+        replay.graph, replay.hands_per_side, replay.static_streams, replay.part_labels = graph, K, streams, labels
+        for name, value in stage.attrs.items():
+            setattr(replay, name, value)
         return replay
 
     @torch.no_grad()

@@ -206,13 +206,19 @@ class RaggedFrames:
             self._stage = torch.empty(size, dtype=torch.uint8, pin_memory=True)
         return self._stage
 
+    def check(self, frames):
+        """Every check of ``load`` -> ``check_ragged``'s (descriptors, offsets, packed bytes, whether the frames are
+        on the host).  Raises TypeError / ValueError; touches no device."""
+        desc, offsets, total, host = check_ragged(frames, self.max_frames, self.max_bytes, self.exact)
+        if not host and any(f.device != self.device for f in frames):
+            raise ValueError(f"CUDA frames must live on {self.device}")
+        return desc, offsets, total, host
+
     def load(self, frames) -> int:
         """Copy a list of (H, W, 3) uint8 BGR frames (numpy arrays or CPU tensors, or CUDA tensors on this device;
         not a mix of host and device frames) into the buffers, on the current stream.  Returns the frame count."""
-        desc, _, total, host = check_ragged(frames, self.max_frames, self.max_bytes, self.exact)
+        desc, _, total, host = self.check(frames)
         n = len(frames)
-        if not host and any(f.device != self.device for f in frames):
-            raise ValueError(f"CUDA frames must live on {self.device}")
         stage = self._staging(self.meta_bytes + (total if host else 0))
         np_stage = stage.numpy()
         np_stage[:n * FRAME_DTYPE.itemsize] = desc.view(np.uint8)
