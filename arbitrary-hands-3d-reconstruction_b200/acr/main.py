@@ -309,10 +309,10 @@ class ACR(nn.Module):
 
     @torch.no_grad()
     def capture_jpeg_graph(self, batch: int, max_coded_bytes: int, max_frame_bytes: int, tracker=None, device=None,
-                           max_blocks: int = None, part_labels=None):
+                           max_blocks: int = None, part_labels=None, max_scans: int = 0):
         """``capture_frames_graph`` from JPEG files: one CUDA graph of the device JPEG decode (acr_b200.jpeg), the
         ragged pre-processing and ``fused_forward``.  Returns ``replay(encoded_list) -> (bufs, mano)`` for exactly
-        ``batch`` baseline JPEG files (bytes-like) whose entropy-coded bytes sum to at most ``max_coded_bytes`` and
+        ``batch`` JPEG files (bytes-like) whose entropy-coded bytes sum to at most ``max_coded_bytes`` and
         whose decoded H*W*3 bytes sum to at most ``max_frame_bytes``; ``max_blocks`` caps the 8x8 coefficient blocks
         (default ``max_frame_bytes // 48 + 64 * batch``: enough for every sampling when each frame is at least 18
         pixels on each side; thin frames pad more per pixel, a 1x1920 frame needs 720 blocks, so give a larger cap).
@@ -322,7 +322,14 @@ class ACR(nn.Module):
         an all-black image; ``replay.jpeg.raise_on_status()`` waits and raises.  Like ``capture_graph``, the graph
         is bound to its ``max_hands_per_side``, and a ``tracker`` is captured with it; with a multi-stream tracker the replay is
         ``replay(encoded_list, stream_ids, stream_begin=None)``.  ``part_labels`` as in ``capture_frames_graph``: True
-        (``max_frame_bytes // 3`` pixels) or a capacity, the labels in ``replay.part_labels``."""
+        (``max_frame_bytes // 3`` pixels) or a capacity, the labels in ``replay.part_labels``.
+
+        With ``max_scans = 0`` the files must be single-scan (baseline or extended sequential); progressive and
+        multi-scan sequential files raise JpegUnsupported.  ``max_scans`` > 0 decodes those on the device too, as long
+        as their scans number at most ``max_scans`` in a replay (single-scan files never count; more raises
+        ValueError naming the capacity).  Every scan's segment starts a decoder chunk of its own, so a file's chunks
+        can exceed its coded bytes / 256 by one per scan: the chunk cap is ``max_coded_bytes / 256 + batch +
+        max_scans``.  The coefficient planes are the frame's whatever the script, so ``max_blocks`` is unchanged."""
         from acr_b200 import jpeg
         from acr_b200.preprocess import RaggedFrames, shapes_layout
         import cv2
@@ -331,8 +338,9 @@ class ACR(nn.Module):
         if max_blocks is None:
             max_blocks = max_frame_bytes // 48 + 64 * batch
         rf = RaggedFrames(batch, max_frame_bytes, dev, args().input_size, exact=True)
-        jb = jpeg.JpegBatch(batch, max_coded_bytes, max_frame_bytes, -(-max_coded_bytes // jpeg.CHUNK) + batch,
-                            max_blocks, dev, out=rf.packed)
+        jb = jpeg.JpegBatch(batch, max_coded_bytes, max_frame_bytes,
+                            -(-max_coded_bytes // jpeg.CHUNK) + batch + max_scans, max_blocks, dev, out=rf.packed,
+                            max_scans=max_scans)
         labels = _label_buffer(part_labels, batch, dev, max_frame_bytes // 3)
 
         def check(encoded_list):

@@ -146,9 +146,11 @@ def img_preprocess(image, imgpath=None, input_size=512, single_img_input=False, 
     return input_data
 
 
-def img_preprocess_jpeg(encoded_list, paths=None, input_size=512, host_fallback=False):
+def img_preprocess_jpeg(encoded_list, paths=None, input_size=512, host_fallback=False, max_scans=0):
     """``img_preprocess`` of a list of JPEG files (encoded bytes): decoded on the device (acr_b200.jpeg.decode, equal
     to cv2.imdecode), then padded and resized in one launch.  Returns the same dict as ``img_preprocess`` of the
-    decoded frames.  Unsupported files raise before anything is enqueued unless ``host_fallback``."""
+    decoded frames.  Unsupported files raise before anything is enqueued unless ``host_fallback``; ``max_scans`` > 0
+    decodes progressive and multi-scan sequential files with up to that many scans in all on the device."""
     from acr_b200 import jpeg
-    return img_preprocess(jpeg.decode(encoded_list, host_fallback=host_fallback), paths, input_size)
+    return img_preprocess(jpeg.decode(encoded_list, host_fallback=host_fallback, max_scans=max_scans), paths,
+                          input_size)

@@ -73,7 +73,8 @@ EXPORTS = ["acr_b200_last_error", "acr_b200_version", "acr_b200_mano_model_float
            "acr_b200_mano_backward_workspace_floats", "acr_b200_mano_backward", "acr_b200_mano_layer_forward",
            "acr_b200_mano_layer_backward", "acr_b200_mano_layer_jvp", "acr_b200_cam_trans", "acr_b200_cam_trans_pnp", "acr_b200_preprocess", "acr_b200_cubic_tables", "acr_b200_preprocess_ragged", "acr_b200_part_labels", "acr_b200_track_state_bytes", "acr_b200_track_hands", "acr_b200_track_streams_workspace_bytes", "acr_b200_track_streams", "acr_b200_rot6d_to_aa", "acr_b200_rodrigues", "acr_b200_parse", "acr_b200_parse_topk",
            "acr_b200_plan_create", "acr_b200_plan_run", "acr_b200_plan_profile", "acr_b200_plan_profile_ops", "acr_b200_plan_num_launches", "acr_b200_plan_op_launch", "acr_b200_plan_destroy",
-           "acr_b200_run_op", "acr_b200_pack_conv", "acr_b200_jpeg_workspace_bytes", "acr_b200_jpeg_coef_offset", "acr_b200_jpeg_decode"]
+           "acr_b200_run_op", "acr_b200_pack_conv", "acr_b200_jpeg_workspace_bytes", "acr_b200_jpeg_coef_offset", "acr_b200_jpeg_decode",
+           "acr_b200_jpeg_scan_workspace_bytes", "acr_b200_jpeg_decode_scans"]
 
 
 def load() -> C.CDLL:
@@ -133,6 +134,10 @@ def load() -> C.CDLL:
     lib.acr_b200_jpeg_coef_offset.restype = C.c_size_t
     lib.acr_b200_jpeg_decode.argtypes = [vp, C.c_int64, vp, i32, C.c_int64, C.c_int64, vp, C.c_size_t, vp, C.c_int64,
                                          vp, vp]
+    lib.acr_b200_jpeg_scan_workspace_bytes.argtypes = [C.c_int64, C.c_int64, C.c_int64]
+    lib.acr_b200_jpeg_scan_workspace_bytes.restype = C.c_size_t
+    lib.acr_b200_jpeg_decode_scans.argtypes = [vp, C.c_int64, vp, i32, vp, C.c_int64, C.c_int64, C.c_int64, vp,
+                                               C.c_size_t, vp, C.c_int64, vp, vp]
     _lib = lib
     return lib
 

@@ -520,7 +520,7 @@ int acr_b200_pack_conv(const float* w_oihw, const float* conv_bias, const float*
                        int cout, int cin, int k, int cout_pad, int cin_pad, int act_dtype,
                        void* w_packed_host, float* bias_host);
 
-/* ---- baseline JPEG decoding (csrc/jpeg.cu) ------------------------------------------------------------------
+/* ---- JPEG decoding (csrc/jpeg.cu) ------------------------------------------------------------------
  * Replaces the host decode of every input mode of the reference (cv2.imread in image / folder mode, and the
  * read-back of the frames split_frame writes in video mode; /root/reference/demo.py, acr/utils.py).  The host parses
  * the headers (acr_b200/jpeg.py) into one acr_b200_jpeg_frame per file; the entropy-coded segments travel
@@ -552,7 +552,9 @@ typedef struct acr_b200_jpeg_frame {
   int32_t comp_bw[3], comp_bh[3]; /* plane size in blocks */
   int32_t comp_w[3], comp_hgt[3]; /* component size in samples (libjpeg's downsampled_width / _height) */
   int32_t comp_block0[3];
-  int32_t reserved;
+  int32_t n_scans; /* 0: a single-scan file; > 0: a multi-scan file decoded from that many acr_b200_jpeg_scan
+                      descriptors (acr_b200_jpeg_decode_scans only): the MCU geometry above is the frame's, restart
+                      and the Huffman tables are unused, and the chunk and coded ranges cover its scans' ranges */
   int8_t slot_comp[8], slot_dy[8], slot_dx[8];
   uint16_t quant[3][64]; /* natural order */
   acr_b200_jpeg_huff dc[3], ac[3];
@@ -580,10 +582,50 @@ size_t acr_b200_jpeg_coef_offset(int64_t max_chunks);
  * other files.  status (device, n int32) gets each frame's ACR_B200_JPEG_* bits; a frame with status != 0 gets an
  * all-black image (none when its descriptor does not fit the buffers, status bit 256).  Every read stays inside the
  * frame's segment, and every store inside its own output.
- * Frames whose descriptor has ncomp == 0 are skipped (left untouched in out_bgr, status 0).                      */
+ * Frames whose descriptor has ncomp == 0 are skipped (left untouched in out_bgr, status 0); a multi-scan frame
+ * (n_scans != 0) gets status 256 here (acr_b200_jpeg_decode_scans decodes it).                                   */
 int acr_b200_jpeg_decode(const uint8_t* coded, int64_t coded_bytes, const acr_b200_jpeg_frame* frames, int n,
                          int64_t max_chunks, int64_t max_blocks, void* workspace, size_t workspace_bytes,
                          uint8_t* out_bgr, int64_t out_bytes, int32_t* status, void* stream);
+
+/* One scan of a progressive (SOF2) or multi-scan sequential (SOF0 / SOF1) file.  Scans of one frame are
+ * consecutive, in file order, and their segments and chunks follow one another inside the frame's ranges.  A scan
+ * with several components (ncomp > 1) is interleaved: it codes the frame's mcus_x x mcus_y MCUs of bpm blocks, block
+ * k of an MCU being component slot_comp[k] at (slot_dy[k], slot_dx[k]) inside it.  A one-component scan codes that
+ * component's own blocks only, mcus_x = ceil(comp_w / 8) by mcus_y = ceil(comp_hgt / 8) in raster order (bpm 1), not
+ * the MCU-padded plane.  restart counts MCUs (blocks of a one-component scan).  First scans (ah == 0: DC first,
+ * AC first, sequential) store coefficients << al; refinement scans (ah != 0, al == ah - 1) add bit al.  dc[c] / ac[c]:
+ * the Huffman tables in force at the scan's SOS for frame component c (those the scan uses).  8632 bytes. */
+typedef struct acr_b200_jpeg_scan {
+  int64_t coded_offset; /* entropy-coded segment: bytes [coded_offset, coded_offset + coded_len) of `coded` */
+  int32_t coded_len;
+  int32_t frame;        /* index of the file in `frames` */
+  int32_t chunk_begin, n_chunks; /* ceil(coded_len / ACR_B200_JPEG_CHUNK) chunks, at least 1 */
+  int32_t ncomp;        /* 1..3 components in the scan; 0: an unused descriptor (after every real one) */
+  int32_t ss, se, ah, al; /* spectral selection and successive approximation (sequential: 0, 63, 0, 0) */
+  int32_t restart;
+  int32_t mcus_x, mcus_y, bpm, n_blocks; /* n_blocks = mcus_x * mcus_y * bpm */
+  int8_t slot_comp[8], slot_dy[8], slot_dx[8];
+  acr_b200_jpeg_huff dc[3], ac[3];
+} acr_b200_jpeg_scan;
+
+/* Workspace of acr_b200_jpeg_decode_scans for at most max_chunks chunks, max_blocks blocks and max_scans scans;
+ * acr_b200_jpeg_coef_offset(max_chunks) is where its coefficient blocks are. */
+size_t acr_b200_jpeg_scan_workspace_bytes(int64_t max_chunks, int64_t max_blocks, int64_t max_scans);
+
+/* acr_b200_jpeg_decode for a batch that may hold multi-scan files (frames with n_scans > 0), described by the
+ * max_scans descriptors at `scans` (device): the real ones first, sorted by frame, then unused ones (ncomp 0,
+ * chunk_begin = the batch's chunk total, frame = INT32_MAX), so a CUDA graph replays with any mix of files.
+ * Single-scan frames decode as in acr_b200_jpeg_decode, in the same launches.  The first scans of every file (DC
+ * first, AC first, sequential) are decoded together with the same speculative chunks, one CTA per scan to
+ * synchronise them; then one CTA per frame applies its refinement scans in file order (one thread walks each scan
+ * to find every block's start from the blocks' nonzero masks, then the CTA decodes the blocks in parallel); then
+ * the IDCT and colour conversion run over every frame.  A multi-scan frame's status is the OR of
+ * its scans' (ACR_B200_JPEG_BAD_LENGTH also when a scan's blocks or EOB run pass its extent). */
+int acr_b200_jpeg_decode_scans(const uint8_t* coded, int64_t coded_bytes, const acr_b200_jpeg_frame* frames, int n,
+                               const acr_b200_jpeg_scan* scans, int64_t max_scans, int64_t max_chunks,
+                               int64_t max_blocks, void* workspace, size_t workspace_bytes, uint8_t* out_bgr,
+                               int64_t out_bytes, int32_t* status, void* stream);
 
 #ifdef __cplusplus
 }
