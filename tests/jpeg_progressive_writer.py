@@ -2,7 +2,10 @@
 (tests/jpeg_writer.py's ``Source``) coded again as several sequential scans (Ss = 0, Se = 63, Ah = Al = 0), each over
 a group of the components, with the source's headers and Huffman tables (``Table`` and the bit writer of
 tests/jpeg_writer.py).  A one-component scan codes the component's own ceil(w / 8) x ceil(h / 8) blocks; an
-interleaved scan codes the frame's MCUs over its components.  ``restart`` sets a DRI before each scan."""
+interleaved scan codes the frame's MCUs over its components.  ``restart`` sets a DRI before each scan; ``fill``
+writes 0xFF fill bytes before each RST and at the end of each scan.  With the default ``fill`` every file is byte for
+byte what the writer wrote before ``fill`` and the feature counters existed (tests/test_cpu_jpeg_progressive_sweep.py
+holds it to digests)."""
 from typing import Sequence
 
 import numpy as np
@@ -37,9 +40,18 @@ def _codes(t):
     return {s: (c, l) for s, (c, l) in JW.Table(t.bits, t.vals).codes().items()}
 
 
-def multi_scan_sequential(buf: bytes, groups: Sequence[Sequence[int]], restart: Sequence[int] = ()) -> bytes:
+def _fill(fill: Sequence[int], k: int) -> bytes:
+    """The 0xFF fill bytes before the k-th RST of a scan (``fill`` cycled); k = -1: before the marker that ends a
+    scan (the first entry)."""
+    return b"\xff" * (fill[k % len(fill)] if k >= 0 else fill[0])
+
+
+def multi_scan_sequential(buf: bytes, groups: Sequence[Sequence[int]], restart: Sequence[int] = (),
+                          fill: Sequence[int] = (0,)) -> bytes:
     """``buf`` (a baseline cv2 file) coded again as one sequential scan per group of component indices, in order.
-    ``restart[k]``: the restart interval of scan k (0 = none; missing = 0)."""
+    ``restart[k]``: the restart interval of scan k (0 = none; missing = 0).  ``fill``: 0xFF fill bytes (T.81
+    B.1.1.2) before each RST, cycling through the list, and ``fill[0]`` of them after each scan, before the next
+    DRI or the EOI."""
     src = JW.source(buf)
     sos = buf.find(b"\xff\xda")
     head = buf[:sos]
@@ -69,12 +81,12 @@ def multi_scan_sequential(buf: bytes, groups: Sequence[Sequence[int]], restart: 
         for u, unit in enumerate(units):
             if rst and u and u % rst == 0:
                 bits.flush()
-                bits.out += bytes([0xFF, 0xD0 + ((u // rst - 1) & 7)])
+                bits.out += _fill(fill, u // rst - 1) + bytes([0xFF, 0xD0 + ((u // rst - 1) & 7)])
                 pred = {c: 0 for c in grp}
             for c, by, bx in unit:
                 pred[c] = _encode_block(bits, src.coef[c][by, bx], pred[c], dc[c], ac[c])
         bits.flush()
-        out += bits.out
+        out += bits.out + _fill(fill, -1)
     out += b"\xff\xd9"
     return bytes(out)
 
@@ -103,10 +115,15 @@ def _bitlen(v: int) -> int:
 
 
 class _Scan:
-    """Events of one scan: ("H", class, comp, symbol), ("B", value, nbits), ("R", marker number)."""
+    """Events of one scan: ("H", class, comp, symbol), ("B", value, nbits), ("R", marker number); ``count``: the
+    stream features of ``STAT_KEYS`` it contains."""
 
     def __init__(self):
         self.ev = []
+        self.count = {}
+
+    def note(self, key):
+        self.count[key] = self.count.get(key, 0) + 1
 
     def huff(self, tc, c, sym):
         self.ev.append(("H", tc, c, sym))
@@ -137,6 +154,7 @@ def _progressive_events(src, comps, ss, se, ah, al, restart):
         n = state["eobrun"]
         if n:
             r = n.bit_length() - 1
+            sc.note(f"eob{r}_{'refine' if ah else 'first'}")
             sc.ev.append(("EOB", r))
             sc.huff(1, comps[0], r << 4)
             sc.bits(n, r)
@@ -148,6 +166,8 @@ def _progressive_events(src, comps, ss, se, ah, al, restart):
     pred = {c: 0 for c in comps}
     for u, unit in enumerate(units):
         if restart and u and u % restart == 0:
+            if state["eobrun"]:
+                sc.note("eobrun_at_rst")
             emit_eobrun()
             sc.ev.append(("R", (u // restart - 1) & 7))
             pred = {c: 0 for c in comps}
@@ -172,6 +192,7 @@ def _progressive_events(src, comps, ss, se, ah, al, restart):
                         continue
                     emit_eobrun()
                     while r > 15:
+                        sc.note("zrl_first")
                         sc.huff(1, c, 0xF0)
                         r -= 16
                     n = mag.bit_length()
@@ -193,6 +214,9 @@ def _progressive_events(src, comps, ss, se, ah, al, restart):
                         continue
                     while r > 15 and k <= eob:
                         emit_eobrun()
+                        sc.note("zrl_refine")
+                        if br:
+                            sc.note("corr_after_zrl")
                         sc.huff(1, c, 0xF0)
                         r -= 16
                         for b in br:
@@ -212,16 +236,30 @@ def _progressive_events(src, comps, ss, se, ah, al, restart):
                     state["be"] += br
                     if state["eobrun"] == 0x7FFF or len(state["be"]) > 937:
                         emit_eobrun()
+    if state["eobrun"]:
+        sc.note("eobrun_at_end")
     emit_eobrun()
     return sc
 
 
-def progressive(buf: bytes, script, restart=None, tables="optimal"):
+STAT_KEYS = (["eob_across", "corr_across", "rst_across", "ff00_across", "max_eobrun", "zrl_first", "zrl_refine",
+              "corr_after_zrl", "eobrun_at_rst", "eobrun_at_end"]
+             + [f"eob{r}_{kind}" for kind in ("first", "refine") for r in range(15)])
+
+
+def progressive(buf: bytes, script, restart=None, tables="optimal", fill: Sequence[int] = (0,)):
     """``buf`` (a baseline cv2 file) coded again as a progressive file with ``script``: a list of
     (component indices, Ss, Se, Ah, Al) in file order.  ``restart[k]``: scan k's restart interval (default none).
-    Every scan gets its own DHT: per-scan ``optimal`` tables or ``long`` ones (codes of 10 to 16 bits).  Returns
-    (file bytes, stats): stats counts the EOBn codes, the correction-bit runs after them, the RST markers and the
-    stuffed FF 00 pairs that straddle a 256-byte boundary of their scan's segment, and the longest EOB run."""
+    Every scan gets its own DHT: per-scan ``optimal`` tables or ``long`` ones (codes of 10 to 16 bits).  ``fill``:
+    0xFF fill bytes before each RST (cycling) and ``fill[0]`` after each scan, before the next DRI / DHT or the EOI.
+    Returns (file bytes, stats), stats over ``STAT_KEYS``:
+      *_across          EOBn codes, the correction-bit runs after them, RST markers and stuffed FF 00 pairs that
+                        straddle a 256-byte boundary of their scan's segment;
+      max_eobrun        the longest EOB run (rounded down to a power of two);
+      zrl_first / zrl_refine   ZRL codes in AC first / AC refinement scans;
+      corr_after_zrl    refinement ZRL codes followed by correction bits;
+      eob{r}_first / eob{r}_refine   EOBn codes of length class r (runs of 2^r .. 2^(r+1) - 1 blocks);
+      eobrun_at_rst / eobrun_at_end  EOB runs cut by a restart marker / ending at the scan's last block."""
     src = JW.source(buf)
     sos = buf.find(b"\xff\xda")
     head = bytearray(buf[:sos])
@@ -230,11 +268,14 @@ def progressive(buf: bytes, script, restart=None, tables="optimal"):
     sel = buf[sos + 5:sos + 5 + 2 * src.ncomp]
     cid = [sel[2 * c] for c in range(src.ncomp)]
     out = bytearray(head)
-    stats = {"eob_across": 0, "corr_across": 0, "rst_across": 0, "ff00_across": 0, "max_eobrun": 0}
+    stats = dict.fromkeys(STAT_KEYS, 0)
     chunk = 256
     for k, (comps, ss, se, ah, al) in enumerate(script):
         rst = restart[k] if restart and k < len(restart) else 0
         sc = _progressive_events(src, comps, ss, se, ah, al, rst)
+        for key, v in sc.count.items():
+            stats[key] += v
+        nres = 0
         freq = {}
         for e in sc.ev:
             if e[0] == "H":
@@ -274,6 +315,8 @@ def progressive(buf: bytes, script, restart=None, tables="optimal"):
                         stats["corr_across"] += 1
             else:
                 bits.flush()
+                bits.out += _fill(fill, nres)
+                nres += 1
                 p = len(bits.out)
                 bits.out += bytes([0xFF, 0xD0 + e[1]])
                 if p // chunk != (p + 1) // chunk:
@@ -281,7 +324,7 @@ def progressive(buf: bytes, script, restart=None, tables="optimal"):
         bits.flush()
         seg = bytes(bits.out)
         stats["ff00_across"] += sum(1 for i in range(chunk - 1, len(seg) - 1, chunk) if seg[i] == 0xFF and seg[i + 1] == 0)
-        out += seg
+        out += seg + _fill(fill, -1)
     out += b"\xff\xd9"
     return bytes(out), stats
 
